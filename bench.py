@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Headline benchmark: BERT-large pre-training throughput (sequences/s, whole job) on N B200s.
+"""Headline benchmark: BERT-large pre-training throughput (sequences/s, whole job) on N H100s.
 
-    python bench.py --gpus 1 --steps K --warmup W                 # this repo (fused sm_100a engine)
+    python bench.py --gpus 1 --steps K --warmup W                 # this repo (fused sm_90a engine)
     python bench.py --impl reference --gpus 1 --steps K --warmup W  # unmodified reference + torch shims
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W    # N > 1, one rank per GPU over NCCL
@@ -26,7 +26,7 @@ and its in-kernel timeline is reported (``extra.fused_step_timeline``).
 
 Timing: W >= 3 untimed warm-up steps, then exactly K steps bracketed by barrier + synchronize, CUDA
 events on the launching stream, max over ranks; an L2 flush (256 MB write) precedes every step and the
-per-step working set (~10 GB of activations) is far larger than the 126 MB L2 anyway; nvidia-smi
+per-step working set (~10 GB of activations) is far larger than the 50 MB L2 anyway; nvidia-smi
 clocks/throttle reasons are sampled during the timed region.
 ``e2e`` repeats the measurement (at most 6 timed steps) through the public training API (`pretrain.forward_backward_pass` /
 `take_optimizer_step`) with every micro-batch copied from pinned host memory inside the timed region and
@@ -79,6 +79,10 @@ def parse():
                     help="RoBERTa-style recipe (seq 512, no NSP, cased vocabulary, linear decay) instead of --phase; ours only")
     ap.add_argument("--kfac", action="store_true", help="K-FAC preconditioner on (BASELINE config #5); ours only")
     ap.add_argument("--seed", type=int, default=42)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps write what the last timed step returned to its caller as DIR/<name>.npy "
+                         "(float32): the loss of every micro-batch and a fixed, seeded sample of the updated fp32 weights "
+                         "and LAMB moments; same arguments -> same inputs, so two builds can be compared output for output")
     return ap.parse_args()
 
 
@@ -158,8 +162,8 @@ def min_over_ranks(x, dev):
 
 
 def fused_parity(comm, arena, opt, dev, rank, world):
-    """Driver-side correctness proof of the fused reduce-scatter + LAMB + all-gather kernel (the driver's pytest box has
-    one GPU): one optimizer step on the REAL arena with per-rank pseudo-random gradients, once as NCCL all-reduce(avg)
+    """Correctness check of the fused reduce-scatter + LAMB + all-gather kernel where several GPUs are at hand (the
+    test suite skips its multi-GPU tests on a single-GPU machine): one optimizer step on the REAL arena with per-rank pseudo-random gradients, once as NCCL all-reduce(avg)
     + single-GPU arena LAMB and once through the peer-memory kernel; returns max |delta| over the bf16 weights every
     rank holds afterwards and the fp32 master shard it owns, max over ranks.  State is restored."""
     import torch
@@ -196,6 +200,22 @@ def fused_parity(comm, arena, opt, dev, rank, world):
     return {"fp32_master_shard": max_over_ranks(d_master, dev), "bf16_weights_all_ranks": max_over_ranks(d_shadow, dev)}
 
 
+def dump_outputs(out_dir, step_losses, arena, sample=1 << 22):
+    """What the last timed optimizer step handed back: its micro-batch losses, and the state it left in the arena
+    (fp32 master weights, LAMB moments) at ``sample`` fixed, seeded positions (3 x 16 MB instead of 3 x 1.3 GB)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    n = arena.flat_param.numel()
+    idx = torch.from_numpy(np.sort(np.random.default_rng(1234).choice(n, size=min(sample, n), replace=False)))
+    idx = idx.to(arena.flat_param.device)
+    arrays = {"loss_per_micro_batch": step_losses, "weights_sample": arena.flat_param[idx],
+              "exp_avg_sample": arena.exp_avg[idx], "exp_avg_sq_sample": arena.exp_avg_sq[idx]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 # ------------------------------------------------------------------------------------------------
 # this repository
 # ------------------------------------------------------------------------------------------------
@@ -208,7 +228,7 @@ def run_ours(args, ph, B, accum, rank, world, dev):
     from bert_pytorch_b200.optim import GradScaler, Lamb, LinearWarmUpScheduler, PolyWarmUpScheduler
     from bert_pytorch_b200.parallel import DataParallel, make_comm
     from bert_pytorch_b200.utils.timing import L2Flusher
-    assert ops.available(), "sm_100a extension not loaded"
+    assert ops.available(), "sm_90a extension not loaded"
     torch.manual_seed(args.seed + rank)
     vocab = ph.get("vocab_size", MODEL["vocab_size"])
     cfg = BertConfig.from_dict(dict(MODEL, vocab_size=vocab, next_sentence=ph.get("next_sentence", True), hidden_act="gelu",
@@ -259,6 +279,7 @@ def run_ours(args, ph, B, accum, rank, world, dev):
     loss_acc = torch.zeros((), device=dev)
 
     opt_events = []
+    step_losses = torch.zeros(accum, device=dev) if args.dump_outputs else None   # micro-batch losses of the latest step
 
     def step_device(i):
         for m in range(accum):
@@ -266,6 +287,8 @@ def run_ours(args, ph, B, accum, rank, world, dev):
             loss = pretrain.forward_backward_pass(ddp, crit, scaler, batch, accum, sync_grads=(m == accum - 1),
                                                   compute_dtype=torch.bfloat16)
             loss_acc.add_(loss)
+            if step_losses is not None:
+                step_losses[m].copy_(loss)
         for sc in scheds:
             sc.step()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -294,6 +317,8 @@ def run_ours(args, ph, B, accum, rank, world, dev):
         parity = fused_parity(comm, arena, opt, dev, rank, world)     # before anything is timed
     l0 = K.KERNEL_LAUNCHES
     ms, clocks = timed_steps(step_device, args.steps, args.warmup, flusher, dev)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step_losses, arena)
     timeline = None
     if world > 1 and hasattr(comm, "timeline") and precond is None:
         torch.cuda.synchronize()
@@ -407,21 +432,15 @@ def run_reference(args, ph, B, accum, rank, world, dev):
 
 def roofline(args, ph, seq_per_s_per_gpu: float) -> dict:
     """Model FLOPs per sequence as executed (GEMMs + attention, forward + backward = 3x forward; the MLM head on the
-    masked rows only for this repo, on every position for the reference) against the MEASURED sustained cuBLAS bf16
-    throughput of this pool (MEASURED_PEAKS.json; the profiling recipe's fallback when the file is absent)."""
+    masked rows only for this repo, on every position for the reference) against the dense bf16 rate of NVIDIA's H100 SXM
+    data sheet (989 TFLOP/s at a 700 W power limit; a whole-program rate over a data-sheet peak, not a kernel's share)."""
     try:
         H, I, L, S = 1024, 4096, args.layers or 24, ph["seq"]
         V = (ph.get("vocab_size", 30522) + 7) // 8 * 8
         head_rows = ph["max_pred"] if args.impl == "ours" else S
         fwd = S * L * (2 * (4 * H * H + 2 * H * I) + 4 * S * H) + head_rows * (2 * H * H + 2 * H * V)
         gflop = 3 * fwd / 1e9
-        peak, src = 1590.0, "fallback"
-        path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-        if os.path.exists(path):
-            with open(path) as f:
-                mp = json.load(f)
-            peak = float(mp.get("bf16_tflops_sustained") or mp.get("bf16_tflops") or peak)
-            src = "MEASURED_PEAKS.json bf16_tflops_sustained"
+        peak, src = 989.0, "H100 SXM data sheet, dense bf16"
         tflops = seq_per_s_per_gpu * gflop / 1e3
         return {"gflop_per_seq": round(gflop, 1), "tflops_per_gpu": round(tflops, 1), "peak_tflops": peak,
                 "peak_source": src, "fraction_of_peak": round(tflops / peak, 3)}
@@ -472,7 +491,7 @@ def run_config(args, rank, world, dev):
                    "mlm_head": "masked-only (max_predictions_per_seq rows per sequence, same loss)" if ours
                    else "dense (every position, as the reference computes it)",
                    "parallelism": f"dp{world}", "grad_reduction": extra.get("backend"),
-                   "l2": "256MB L2 flush before every step; per-step working set (~10 GB activations) >> 126 MB L2",
+                   "l2": "256MB L2 flush before every step; per-step working set (~10 GB activations) >> 50 MB L2",
                    "note": "step = one optimizer step of accumulation_steps micro-batches incl. gradient reduction + LAMB; "
                            "default accumulation = shipped global batch on 8 GPUs (per-GPU work fixed: weak scaling)"},
         "clocks": {"sm_mhz": clocks.get("sm_mhz"), "sm_max_mhz": clocks.get("sm_max_mhz"),
@@ -506,11 +525,14 @@ def main():
     args = parse()
     if args.impl == "reference" and not os.path.exists(os.path.join(ROOT, "baseline", "_ref", "run_pretraining.py")):
         print(json.dumps({"impl": "reference", "unavailable": "baseline/_ref missing: the reference has no "
-                          "setup.py/pyproject.toml so pip cannot install it; copy /root/reference there"}))
+                          "setup.py/pyproject.toml so pip cannot install it; put a copy of its tree there"}))
         return
     import torch
     if not torch.cuda.is_available():
         print(json.dumps({"impl": args.impl, "unavailable": "no CUDA device"}))
+        return
+    if args.dump_outputs and args.impl != "ours":
+        print(json.dumps({"impl": args.impl, "unavailable": "--dump-outputs is implemented for this repository's arm only"}))
         return
     if (args.roberta or args.kfac) and args.impl != "ours":
         print(json.dumps({"impl": args.impl, "unavailable": "--roberta / --kfac are measured for this repository only "
@@ -558,7 +580,7 @@ def main():
         configs = state["configs"] = {}
         for name, over in subs:
             sub = argparse.Namespace(**vars(args))
-            sub.steps, sub.warmup, sub.no_e2e, sub.global_batch = min(args.steps, 4), 3, True, 0
+            sub.steps, sub.warmup, sub.no_e2e, sub.global_batch, sub.dump_outputs = min(args.steps, 4), 3, True, 0, None
             for k, v in over.items():
                 setattr(sub, k, v)
             gc.collect()

@@ -1,9 +1,9 @@
-"""bert_pytorch_b200 -- a Blackwell (sm_100a) native BERT pretraining / finetuning stack.
+"""bert_pytorch_b200 -- a Hopper (sm_90a) native BERT pretraining / finetuning stack.
 
 Layout
 ------
 models/    BertConfig, the nn.Module model zoo (state-dict compatible with the
-           reference, SURVEY.md 2.5.3) and the fused sm_100a execution engine
+           reference, SURVEY.md 2.5.3) and the fused sm_90a execution engine
 ops/       hand written CUDA kernels (csrc/) + their Python bindings
 optim/     LAMB / Adam (fused multi-tensor kernels + pure-torch oracles),
            LR schedulers, gradient scaler

@@ -11,7 +11,7 @@ Parity targets (reference file:line):
     index space per rank, is its own iterator, ``state_dict`` = ``{epoch, seed,
     num_replicas, total_size, index}`` with the changed-size / changed-world guards.
 
-Design differences (B200-first; a B200 eats ~3k sequences/s so the reference's
+Design differences (H100-first; an H100 eats ~3k sequences/s so the reference's
 per-token Python loop x 4 DataLoader workers per rank cannot feed eight of them):
   * masking is vectorised over the whole micro-batch (:func:`mask_batch`, numpy here,
     multi-threaded C++ in ops/csrc/host.cpp when built) and writes straight into pinned

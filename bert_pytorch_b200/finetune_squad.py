@@ -7,7 +7,7 @@ Flags, outputs and metrics follow the reference's run_squad.py (:732-857, :1115-
 ``inference_sequences_per_second``, ``exact_match``, ``F1``; the feature cache pickle is named
 ``<train>_<bert_model>_<max_seq>_<stride>_<max_query>``.
 
-Execution differs (B200-first): the encoder runs through the fused sm_100a engine behind an autograd
+Execution differs (H100-first): the encoder runs through the fused sm_90a engine behind an autograd
 bridge; ``--fp16``/``--amp`` select 16-bit compute (bf16 by default on CUDA -- no loss scaling needed;
 ``--loss_scale`` is honoured for fp16) with the fused multi-tensor Adam kernel (apex FusedAdam contract,
 ``bias_correction=False``) on the flat arena and device-side gradient clipping (no ``.item()`` per

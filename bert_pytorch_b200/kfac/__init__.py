@@ -24,8 +24,8 @@ as gradient workers per layer.  Collectives go through the repo's ``Comm`` inter
 gloo / NCCL / peer-memory transport as the gradient reduction.
 
 Where the activations come from: on the plain-PyTorch path forward-pre / backward hooks on the ``nn.Linear``
-modules (``compute_factor_in_hook``); on the fused sm_100a path the engine hands the very tensors it already
-saved for backward to :meth:`KFAC.tap`, and the factor SYRKs run on the tcgen05 GEMM (TN layout, fp32 out).
+modules (``compute_factor_in_hook``); on the fused sm_90a path the engine hands the very tensors it already
+saved for backward to :meth:`KFAC.tap`, and the factor SYRKs run on the wgmma GEMM (TN layout, fp32 out).
 Registered: ``nn.Linear`` layers whose class/name path does not match ``skip_layers`` (Q, K, V, attention
 output, FFN output, NSP) -- ``LinearActivation`` layers (FFN-in, pooler, MLM transform) are not, matching what
 kfac_pytorch's module-type registry would do with this model.
@@ -68,7 +68,7 @@ class _Layer:
 
 
 def _factor(x: torch.Tensor) -> torch.Tensor:
-    """x^T x in fp32 -- tcgen05 TN GEMM on CUDA bf16 inputs, torch elsewhere."""
+    """x^T x in fp32 -- wgmma TN GEMM on CUDA bf16 inputs, torch elsewhere."""
     if x.is_cuda and x.dtype == torch.bfloat16 and x.size(1) % 8 == 0:
         from .. import ops
         if ops.available():

@@ -7,7 +7,7 @@ CUDA -- a bf16 shadow copy of the weights that the tensor-core kernels read.  Th
 2.5.3) but become *views* into the arena, and ``param.grad`` is a persistent view into
 ``flat_grad``.
 
-Why (B200-first, SURVEY.md 7.1 / 5.8):
+Why (H100-first, SURVEY.md 7.1 / 5.8):
   * the optimizer is three launches over contiguous memory instead of 398 tensors,
   * the gradient all-reduce (NCCL baseline or the fused peer-memory kernel) and the
     partitioned LAMB update work on plain ``[offset, offset+n)`` shards,

@@ -1,16 +1,16 @@
-"""Fused sm_100a execution engine for the BERT encoder and the pre-training heads.
+"""Fused sm_90a execution engine for the BERT encoder and the pre-training heads.
 
 The ``nn.Module`` tree in :mod:`.modeling` only *holds* the parameters (as views into the
-:class:`~.arena.ParamArena`); on a B200 the math runs here as an explicit forward/backward
+:class:`~.arena.ParamArena`); on an H100 the math runs here as an explicit forward/backward
 *kernel program* -- no autograd graph, no per-op Python dispatch beyond one launch per fused block:
 
   embeddings   gather x3 + add + LayerNorm + dropout                       1 kernel   (K1-K3)
-  per layer    QKV GEMM [M,H]x[H,3H] + bias                                 tcgen05    (K5, K6 gone)
-               flash attention (scale, key-padding, softmax, dropout, PV)   tcgen05    (K7-K12)
-               out-proj GEMM + bias + dropout + residual                    tcgen05    (K13-K14)
+  per layer    QKV GEMM [M,H]x[H,3H] + bias                                 wgmma    (K5, K6 gone)
+               flash attention (scale, key-padding, softmax, dropout, PV)   wgmma    (K7-K12)
+               out-proj GEMM + bias + dropout + residual                    wgmma    (K13-K14)
                LayerNorm                                                     1 kernel   (K15)
-               FFN-1 GEMM + bias + GELU (and GELU' for the backward) epilogue  tcgen05    (K16)
-               FFN-2 GEMM + bias + dropout + residual                        tcgen05    (K17-K18)
+               FFN-1 GEMM + bias + GELU (and GELU' for the backward) epilogue  wgmma    (K16)
+               FFN-2 GEMM + bias + dropout + residual                        wgmma    (K17-K18)
                LayerNorm                                                     1 kernel
   MLM head     compact masked positions -> gather -> transform GEMM+GELU -> LN -> decoder GEMM + bias
                -> softmax-CE fwd+bwd in place (only max_pred rows/sequence, K21-K24; fixes Q15)
@@ -22,7 +22,7 @@ The ``nn.Module`` tree in :mod:`.modeling` only *holds* the parameters (as views
 
 Dropout masks are a counter-based function of (seed, stream id, element index) so backward regenerates
 them (nothing stored, and recompute is deterministic -- SURVEY.md K27).
-Activations are saved rather than recomputed by default: a B200 has 180 GB (phase-1 micro-batch 96x128 needs
+Activations are saved rather than recomputed by default: an H100 has 80 GB (phase-1 micro-batch 96x128 needs
 ~10 GB); ``--checkpoint_activations`` replays ceil(sqrt(L))-layer segments instead.
 Options: fp8 GEMM operands (``enable_fp8`` / ``B200_FP8=1`` / ``--fp8``), whole-micro-step CUDA-graph replay
 (``FusedPretrainer``, on by default, ``B200_GRAPH=0`` disables), K-FAC taps.
@@ -356,11 +356,11 @@ class FusedEncoderEngine:
             ctx = ctx.view(M, H)
             ctx_q = q[0].view(M, H) if q else None
         # keep bits of the hidden dropout leave the GEMM epilogue (1 bit per element) so that the LayerNorm backward does
-        # not have to run Philox again (60 of its 290 instructions per 8 elements) -- CTA-pair kernel, bf16 path only
-        keep_bits = (save and ph > 0 and not self.fp8 and H % 128 == 0 and K.pick_block_n(M, H) == 512
+        # not have to run Philox again -- bf16 path only
+        keep_bits = (save and ph > 0 and not self.fp8 and H % 128 == 0
                      and os.environ.get("B200_DROP_MASK", "1") != "0")
         # ... and are GENERATED by their own kernel (K.dropout_mask: every warp of the machine on Philox) rather than by
-        # the two epilogue warps per SMSP of the GEMM: 9.6 k of the 13.6 k cycles per tile of that epilogue were Philox
+        # the GEMM's epilogue warps while the tensor cores idle
         mask1 = K.dropout_mask(M, H, ph, seed, _stream(l, SITE_ATTN_OUT), x.device) if keep_bits else None
         mask2 = K.dropout_mask(M, H, ph, seed, _stream(l, SITE_FFN_OUT), x.device) if keep_bits else None
         pre1, ctx_op = self._lin(l, "ctx", "wo", ctx, self.w(pre + "attention.output.dense.weight"), xq=ctx_q,
@@ -551,7 +551,7 @@ class _EncoderFn(torch.autograd.Function):
 
 class _HeadLinearFn(torch.autograd.Function):
     """y = x W^T + b for the small-N fine-tuning heads (QA: N = 2, token / sequence classifiers: N = num_labels,
-    multiple choice: N = 1; reference src/modeling.py:1127-1128, 1188-1189, 1256-1257, 1323-1326) on the tcgen05 GEMM:
+    multiple choice: N = 1; reference src/modeling.py:1127-1128, 1188-1189, 1256-1257, 1323-1326) on the wgmma GEMM:
     N is padded to 8 output columns, forward NT with fp32 store, dgrad NN, wgrad TN with fp32 store -- the SQuAD / NER
     steps then contain no library GEMM (VERDICT r1: K28 / K29 ran as torch ops = cuBLAS behind the bridge)."""
 
@@ -585,7 +585,7 @@ class _HeadLinearFn(torch.autograd.Function):
 
 
 def head_linear(linear: torch.nn.Linear, x: torch.Tensor) -> torch.Tensor:
-    """``linear(x)`` through :class:`_HeadLinearFn` when the sm_100a extension can serve it (CUDA, H % 8 == 0, at most
+    """``linear(x)`` through :class:`_HeadLinearFn` when the sm_90a extension can serve it (CUDA, H % 8 == 0, at most
     64 outputs, at least 128 rows -- smaller problems are launch bound either way), else the module itself."""
     H = x.size(-1)
     rows = x.numel() // max(H, 1)
@@ -736,7 +736,7 @@ class FusedPretrainer:
         d_seq = torch.zeros(M, H, dtype=torch.bfloat16, device=seq.device)
         K.scatter_rows(d_rows, idx, d_seq)
 
-        # ---- NSP head on our own kernels as well (K19 / K20 / K25): pooler = tcgen05 GEMM with the bias+tanh epilogue
+        # ---- NSP head on our own kernels as well (K19 / K20 / K25): pooler = wgmma GEMM with the bias+tanh epilogue
         #      on the [CLS] rows, classifier + CE + their backward = one small kernel, pooler backward = the usual
         #      dgrad / wgrad GEMMs (M = B rows)
         if self.has_nsp and next_sentence_labels is not None:

@@ -3,10 +3,10 @@
 The modules below carry the parameters under exactly the state-dict names of the
 reference (SURVEY.md 2.5.3; src/modeling.py:338-617, 802-1327) so checkpoints
 move freely between the two code bases.  Each module has a plain-PyTorch
-``forward`` that is the numerics oracle and the CPU / gloo execution path.  On a
-B200 the encoder + pre-training heads do not run these forwards: ``BertModel``
+``forward`` that is the numerics oracle and the CPU / gloo execution path.  On an
+H100 the encoder + pre-training heads do not run these forwards: ``BertModel``
 hands the whole encoder to :mod:`bert_pytorch_b200.models.fused`, which executes
-hand written sm_100a kernels straight out of the flat parameter arena.
+hand written sm_90a kernels straight out of the flat parameter arena.
 
 Numerics contract (SURVEY.md appendix B): LayerNorm eps 1e-12 inside the sqrt with
 fp32 statistics, erf-GELU, attention scale applied after QK^T, additive -10000
@@ -382,7 +382,7 @@ class BertPreTrainedModel(nn.Module):
 
     def enable_apex(self, val: bool) -> None:
         """Kept for CLI compatibility (src/modeling.py:653-657); selects the fused
-        sm_100a LayerNorm/engine path instead of apex."""
+        sm_90a LayerNorm/engine path instead of apex."""
         for m in self.modules():
             if isinstance(m, BertModel):
                 m.use_fused = bool(val)
@@ -503,7 +503,7 @@ class BertModel(BertPreTrainedModel):
         self.encoder = BertEncoder(config)
         self.pooler = BertPooler(config) if getattr(config, "next_sentence", True) else None
         self.output_all_encoded_layers = bool(getattr(config, "output_all_encoded_layers", False))
-        self.use_fused = True   # the sm_100a engine is used whenever it can be
+        self.use_fused = True   # the sm_90a engine is used whenever it can be
         self._engine = None
         self.apply(self.init_bert_weights)
 
@@ -514,7 +514,7 @@ class BertModel(BertPreTrainedModel):
         return (1.0 - m) * -10000.0
 
     def fused_engine(self):
-        """The sm_100a execution engine bound to this module's parameters (built
+        """The sm_90a execution engine bound to this module's parameters (built
         lazily the first time a CUDA forward is requested)."""
         if self._engine is None:
             from .fused import FusedEncoderEngine
@@ -522,7 +522,7 @@ class BertModel(BertPreTrainedModel):
         return self._engine
 
     def fusable_config(self) -> bool:
-        """Whether the sm_100a kernel program implements this configuration.  The reference model runs any
+        """Whether the sm_90a kernel program implements this configuration.  The reference model runs any
         ``hidden_act`` of ``ACT2FN`` and any head size (src/modeling.py:118-139); the fused engine is specialised for
         erf-GELU and head_dim 64 with H a multiple of 64 and S <= 512 -- everything else takes the plain PyTorch path
         instead of raising (VERDICT r1, missing #4)."""
@@ -579,7 +579,7 @@ class BertForPreTraining(BertPreTrainedModel):
         return self.cls(seq, pooled)
 
     def pretrain_engine(self):
-        """The fused sm_100a forward+backward engine for MLM(+NSP) training, or ``None`` when the
+        """The fused sm_90a forward+backward engine for MLM(+NSP) training, or ``None`` when the
         model is not on a CUDA device / fusion is disabled (then the autograd path runs)."""
         if not self.bert.use_fused or not self.bert.fusable_config():
             return None                   # e.g. relu / swish FFN or head_dim != 64: the autograd oracle path trains it
@@ -669,7 +669,7 @@ class BertForMultipleChoice(BertPreTrainedModel):
 
 
 def _head(linear: nn.Linear, x: torch.Tensor) -> torch.Tensor:
-    """Small-N head projection: the tcgen05 GEMM path on CUDA (models/fused.py:head_linear), ``linear(x)`` elsewhere."""
+    """Small-N head projection: the wgmma GEMM path on CUDA (models/fused.py:head_linear), ``linear(x)`` elsewhere."""
     if x.is_cuda:
         from .fused import head_linear
         return head_linear(linear, x)
@@ -691,7 +691,7 @@ class BertForTokenClassification(BertPreTrainedModel):
     def forward(self, input_ids, token_type_ids=None, attention_mask=None, labels=None):
         layers, _ = self.bert(input_ids, token_type_ids, attention_mask)
         seq = layers[-1]
-        logits = _head(self.classifier, self.dropout(seq))          # K29: own small-N GEMM on a B200
+        logits = _head(self.classifier, self.dropout(seq))          # K29: own small-N GEMM on an H100
         if labels is not None:
             flat_logits = logits.view(-1, self.num_labels).float()
             flat_labels = labels.view(-1)
@@ -712,7 +712,7 @@ class BertForQuestionAnswering(BertPreTrainedModel):
     def forward(self, input_ids, token_type_ids=None, attention_mask=None):
         layers, _ = self.bert(input_ids, token_type_ids, attention_mask)
         seq = layers[-1]
-        logits = _head(self.qa_outputs, seq)                        # K28: own small-N GEMM on a B200
+        logits = _head(self.qa_outputs, seq)                        # K28: own small-N GEMM on an H100
         start, end = logits.split(1, dim=-1)
         return start.squeeze(-1), end.squeeze(-1)
 

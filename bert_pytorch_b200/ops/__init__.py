@@ -1,4 +1,4 @@
-"""Hand written sm_100a kernels and their bindings.
+"""Hand written sm_90a kernels and their bindings.
 
 ``available()`` is true when a CUDA device is present *and* the in-tree extension
 ``_C.so`` (built by :mod:`bert_pytorch_b200.ops.build`, sources in ``csrc/``) loads.  On a GPU
@@ -49,7 +49,7 @@ def available() -> bool:
         if os.environ.get("B200_ALLOW_EAGER") == "1":
             return False
         raise RuntimeError(
-            f"CUDA device present but the sm_100a extension failed to load: {_ERR!r}. Refusing to "
+            f"CUDA device present but the sm_90a extension failed to load: {_ERR!r}. Refusing to "
             "fall back to eager PyTorch silently (export B200_ALLOW_EAGER=1 to allow it).")
     return True
 

@@ -1,4 +1,4 @@
-"""Python wrappers over the sm_100a extension (``_C.so``).
+"""Python wrappers over the sm_90a extension (``_C.so``).
 
 Thin: allocate outputs, pick tile/split heuristics, translate enums.  No autograd here -- the
 fused engine (models/fused.py) calls forward and backward kernels explicitly.
@@ -14,26 +14,17 @@ import torch
 
 from . import extension
 
-# GEMM enums (csrc/gemm_sm100.h)
+# GEMM enums (csrc/gemm_sm90.h)
 NT, NN, TN = 0, 1, 2
 (EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROP_RES, EPI_ADD, EPI_DGELU, EPI_ACCUM_F32, EPI_BIAS_TANH, EPI_F32,
  EPI_BIAS_GELU_DG, EPI_MUL) = range(11)
 
-NUM_SMS = 148
-_PAIR_ENABLED = os.environ.get("B200_GEMM_PAIR", "1") != "0"
+NUM_SMS = 132           # H100 SXM; only the tile heuristics below use it (the kernels ask the device)
 KERNEL_LAUNCHES = 0     # every wrapper bumps this: bench.py reports it as ``gpu_launches``
 
 
-# stream-K weight gradients: measured slower than 2-4 way split-K on the BERT-large shapes (operands of
-# neighbouring clusters stop sharing L2 lines: profiles/gemm_bench_r1_v3_streamk.jsonl), so opt-in
-STREAM_K = os.environ.get("B200_STREAM_K", "0") == "1"
-# tail split (idle CTA pairs take the K tails): +3 % on the 48-tile QKV weight gradient, -8 % on the 64-tile FFN
-# ones (each helper pays one fp32 red epilogue per tail piece) -> opt-in as well
-TAIL_SPLIT = os.environ.get("B200_TAIL_SPLIT", "0") == "1"
-
-
 def pick_block_n(M: int, N: int) -> int:
-    """The tile variant :func:`gemm` chooses for an [M, N] output (512 = CTA-pair kernel)."""
+    """The tile width :func:`gemm` chooses for an [M, N] output (128 x 256 or 128 x 128 tiles)."""
     return _pick_block_n(M, N)
 
 
@@ -43,20 +34,18 @@ def _count(n: int = 1) -> None:
 
 
 def _pick_block_n(M: int, N: int) -> int:
-    """512 = CTA-pair kernel (256 x 256 tile per 2-CTA cluster, tcgen05 cta_group::2): the default for the
-    large GEMMs; 256 / 128 = single-CTA 128 x N tiles for small or skinny problems."""
-    if M > 128 and N > 128 and _PAIR_ENABLED:
-        return 512
+    """256 (128 x 256 tiles: half the A-operand traffic per FLOP) unless the narrow tiles waste clearly fewer SM
+    slots in the last wave; 128 for N <= 128."""
     if N <= 128:
         return 128
     m_blocks = (M + 127) // 128
     t256 = m_blocks * ((N + 255) // 256)
     t128 = m_blocks * ((N + 127) // 128)
 
-    def eff(tiles: int, width: int) -> float:
+    def eff(tiles: int) -> float:
         waves = math.ceil(tiles / NUM_SMS)
-        return tiles * width / (waves * NUM_SMS * width) if tiles else 0.0
-    return 256 if eff(t256, 256) >= eff(t128, 128) - 0.08 else 128
+        return tiles / (waves * NUM_SMS) if tiles else 0.0
+    return 256 if eff(t256) >= eff(t128) - 0.08 else 128
 
 
 def gemm(a: torch.Tensor, b: torch.Tensor, *, layout: int = NT, epi: int = EPI_NONE,
@@ -67,11 +56,11 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, layout: int = NT, epi: int = EPI_N
          a_e5m2: bool = False, b_e5m2: bool = False, push: bool = False,
          colsum: Optional[torch.Tensor] = None, mask_out: Optional[torch.Tensor] = None,
          mask_in: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """tcgen05 GEMM with a fused epilogue (see csrc/gemm_sm100.cu).  ``a``/``b`` are 2-D bf16, or -- with
+    """wgmma GEMM with a fused epilogue (see csrc/gemm_sm90.cu).  ``a``/``b`` are 2-D bf16, or -- with
     ``scale_a``/``scale_b`` (device inv-scale scalars from an :class:`Fp8Meta`) -- 1-byte fp8 tensors.
     ``colsum`` (fp32 [N], EPI_NONE / EPI_ADD / EPI_MUL): accumulates the column sums of the bf16 output (a bias
     gradient that would otherwise need its own pass over the tensor).  ``mask_out`` (uint8 [M, N / 8],
-    EPI_BIAS_DROP_RES on the CTA-pair kernel): receives the dropout keep bits, which :func:`layer_norm_bwd` can read
+    EPI_BIAS_DROP_RES): receives the dropout keep bits, which :func:`layer_norm_bwd` can read
     back (``keep_mask``) instead of regenerating them."""
     if layout == NT:
         M, N = a.size(0), b.size(0)
@@ -82,43 +71,10 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, layout: int = NT, epi: int = EPI_N
     if out is None:
         dt = torch.float32 if epi in (EPI_ACCUM_F32, EPI_F32) else torch.bfloat16
         out = torch.empty(M, N, dtype=dt, device=a.device)
-    if scale_a is not None:
-        block_n = 512                      # fp8 operands run on the CTA-pair kernel
-    elif block_n is None:
+    if block_n is None:
         block_n = _pick_block_n(M, N)
     extension().gemm(a, b, out, layout, epi, bias, res, aux_out, k_splits, block_n, alpha, p_drop, seed, stream,
                      scale_a, scale_b, a_e5m2, b_e5m2, push, colsum, mask_out, mask_in)
-    _count()
-    return out
-
-
-def mx_quantize(x: torch.Tensor):
-    """bf16 [R, K] -> (e4m3 bytes [R, K], ue8m0 block scales in the tensor-core layout): OCP MXFP8, one scale per
-    32 elements along K (csrc/gemm_mx.cu)."""
-    R, Kd = x.shape
-    q = torch.empty(R, Kd, dtype=torch.uint8, device=x.device)
-    sf = torch.empty(((R + 127) // 128) * (Kd // 128) * 512, dtype=torch.uint8, device=x.device)
-    extension().mx_quantize(x, q, sf)
-    _count()
-    return q, sf
-
-
-def mx_dequantize(q: torch.Tensor, sf: torch.Tensor) -> torch.Tensor:
-    """fp32 view of an MXFP8 tensor (test / debugging aid; plain torch)."""
-    R, Kd = q.shape
-    rows = torch.arange(R, device=q.device)
-    groups = torch.arange(Kd // 32, device=q.device)
-    idx = ((rows[:, None] // 128) * (Kd // 128) + groups[None, :] // 4) * 512 + (rows[:, None] % 32) * 16 \
-        + ((rows[:, None] // 32) % 4) * 4 + groups[None, :] % 4
-    scale = torch.exp2(sf.long()[idx].float() - 127.0)                    # [R, K/32]
-    return q.view(torch.float8_e4m3fn).float() * scale.repeat_interleave(32, dim=1)
-
-
-def gemm_mx(a_q: torch.Tensor, a_sf: torch.Tensor, b_q: torch.Tensor, b_sf: torch.Tensor, *,
-            bias: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
-    """D = A . B^T on block-scaled fp8 operands (tcgen05.mma.kind::mxf8f6f4.block_scale, scales staged in TMEM)."""
-    out = torch.empty(a_q.size(0), b_q.size(0), dtype=out_dtype, device=a_q.device)
-    extension().gemm_mxfp8(a_q, a_sf, b_q, b_sf, out, bias)
     _count()
     return out
 
@@ -167,21 +123,11 @@ class Fp8Meta:
         _count()
 
 
-# opt-in: 256 x 512 weight-gradient tiles measured faster in isolation (0.088 vs 0.096 ms, FFN shapes) but slower inside
-# the training step (74.5 vs 62.9 us per call, side stream off) -- profiles/README.md
-WGRAD_WIDE = os.environ.get("B200_WGRAD_WIDE", "0") == "1"
-
-
 def wgrad_splits(n_out: int, k_out: int, reduce_len: int, block_n: int = 256) -> int:
     """Split-K factor for dW[n_out, k_out] so the grid covers the machine."""
-    if block_n == 512:
-        tiles = ((n_out + 255) // 256) * ((k_out + 255) // 256)
-        units = NUM_SMS // 2
-    else:
-        tiles = ((n_out + 127) // 128) * ((k_out + block_n - 1) // block_n)
-        units = NUM_SMS
+    tiles = ((n_out + 127) // 128) * ((k_out + block_n - 1) // block_n)
     kb = max(1, (reduce_len + 63) // 64)
-    want = max(1, round(2 * units / max(tiles, 1)))
+    want = max(1, round(2 * NUM_SMS / max(tiles, 1)))
     return max(1, min(want, kb // 4 if kb >= 8 else 1, 32))
 
 
@@ -189,42 +135,8 @@ def wgrad_accumulate(dy: torch.Tensor, x: torch.Tensor, grad: torch.Tensor, alph
                      **fp8) -> None:
     """grad[N,K] (fp32, arena view) += dy[M,N]^T @ x[M,K]  (``fp8``: scale_a / scale_b / a_e5m2 for 1-byte operands)."""
     n_out, k_out = grad.shape
-    bn = 512 if fp8 else _pick_block_n(n_out, k_out)
-    if bn == 128 and k_out >= 256:
-        bn = 256
-    if bn == 512 and not fp8 and WGRAD_WIDE and k_out % 512 == 0:
-        # 256 x 512 tiles (two N = 256 MMAs per k-step share the A operand: a quarter fewer operand bytes per FLOP, which
-        # is what the MN-major TMA supply of the TN kernel is short of); fewer tiles than CTA pairs -> tail split
-        tiles = ((n_out + 255) // 256) * (k_out // 512)
-        kb = (dy.size(0) + 63) // 64
-        pairs = NUM_SMS // 2
-        splits = -2 if (tiles < pairs and kb * tiles // pairs >= 4) else 1
-        gemm(dy, x, layout=TN, epi=EPI_ACCUM_F32, out=grad, block_n=1024, alpha=alpha, k_splits=splits, push=push)
-        return
+    bn = 256 if k_out >= 256 else _pick_block_n(n_out, k_out)
     splits = wgrad_splits(n_out, k_out, dy.size(0) // (2 if fp8 else 1), bn)
-    if bn == 512 and not fp8 and not TAIL_SPLIT and not STREAM_K:
-        # round-2 measurement with the 7-stage operand ring (profiles/gemm_bench_r2_wgrad.jsonl): the 48-tile QKV
-        # weight gradient gains 6 % from the tail split (1179 vs 1110 TFLOP/s), the 64-tile FFN ones lose 18 %
-        tiles = ((n_out + 255) // 256) * ((k_out + 255) // 256)
-        if 40 <= tiles <= 56:
-            splits = -2
-    if bn == 512 and TAIL_SPLIT:
-        # fewer tiles than CTA pairs and a split-K grid that leaves > 7 % of the machine idle in its last wave:
-        # tail split (cluster t runs the head of tile t's K range, the idle clusters share the tails; gemm_sm100.cu)
-        tiles = ((n_out + 255) // 256) * ((k_out + 255) // 256)
-        pairs = NUM_SMS // 2
-        kb = (dy.size(0) + (127 if fp8 else 63)) // (128 if fp8 else 64)
-        if tiles < pairs:
-            units = tiles * max(splits, 1)
-            eff = units / (((units + pairs - 1) // pairs) * pairs)
-            if eff < 0.93 and kb * tiles // pairs >= 4:
-                splits = -2
-    if bn == 512 and STREAM_K:
-        # stream-K: equal (tile, k-block) ranges per CTA pair instead of whole tiles (csrc/gemm_sm100.cu: seg_get)
-        tiles = ((n_out + 255) // 256) * ((k_out + 255) // 256)
-        kb = (dy.size(0) + (127 if fp8 else 63)) // (128 if fp8 else 64)
-        if tiles % (NUM_SMS // 2) != 0 and tiles * kb >= 8 * (NUM_SMS // 2):
-            splits = -1
     # ``push``: with the peer-memory backend in push mode the tiles go to the owner rank's arena (GEMM -> reduce-scatter)
     gemm(dy, x, layout=TN, epi=EPI_ACCUM_F32, out=grad, block_n=bn, alpha=alpha, k_splits=splits, push=push, **fp8)
 
@@ -391,19 +303,12 @@ def attention_bwd(qkv, seqlens, ctx, dctx, lse, heads: int, *, p_drop=0.0, seed=
     H = H3 // 3
     dqkv = torch.empty_like(qkv)
     delta = torch.empty(B, heads, S, dtype=torch.float32, device=qkv.device)
-    dq_acc = torch.empty(B * S, H, dtype=torch.float32, device=qkv.device) if S > 128 else None
+    dq_acc = torch.empty(B * S, H, dtype=torch.float32, device=qkv.device)
     q, rec, e5 = _fp8_side(fp8, dqkv)
     extension().attention_bwd(qkv, seqlens, ctx, dctx, lse, dqkv, delta, dq_acc, heads, 1.0 / math.sqrt(H // heads), p_drop,
                               seed, stream, q, rec, e5)
     _count(2)
     return dqkv if fp8 is None else (dqkv, q)
-
-
-def set_attention_options(bwd_pipe: Optional[bool] = None, row_kernels: Optional[bool] = None) -> None:
-    """``bwd_pipe``: force the software-pipelined S > 128 backward kernel on / off; ``row_kernels``: force the
-    round-2 thread-per-query-row kernels on / off (None: follow B200_ATTN_BWD_PIPE / B200_ATTN_ROW, both default on)."""
-    extension().set_attention_options(-1 if bwd_pipe is None else int(bool(bwd_pipe)),
-                                      -1 if row_kernels is None else int(bool(row_kernels)))
 
 
 # ---------------------------------------------------------------------------

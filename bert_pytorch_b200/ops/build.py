@@ -1,4 +1,4 @@
-"""In-tree build of the native code (run on the CPU box; nvcc cross-compiles sm_100a):
+"""In-tree build of the native code (needs no GPU: nvcc cross-compiles for sm_90a):
 
     python -m bert_pytorch_b200.ops.build            # everything
     python -m bert_pytorch_b200.ops.build --host     # only the host helper
@@ -6,7 +6,7 @@
 Produces ``ops/_C.so`` (CUDA kernels + torch bindings) and ``ops/_host.so`` (HDF5 chunk inflate +
 dynamic masking, plain C++).  The kernels are compiled with plain nvcc (no torch headers -> seconds
 per file) and only ``bindings.cpp`` sees torch; objects are cached by source hash under
-``ops/_build``.  The ``.so`` files are git-ignored but travel with ``gpurun`` snapshots.
+``ops/_build``.  The ``.so`` files and ``ops/_build`` are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -23,11 +23,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "_build")
 
-CUDA_SOURCES = ["gemm_sm100.cu", "norm_embed.cu", "optim.cu", "loss.cu", "attention.cu", "comm.cu", "fp8.cu", "gemm_mx.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+CUDA_SOURCES = ["gemm_sm90.cu", "norm_embed.cu", "optim.cu", "loss.cu", "attention_sm90.cu", "comm.cu", "fp8.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # erff/expf accuracy matters for GELU and softmax statistics -> no fast-math there
-PRECISE = {"gemm_sm100.cu", "norm_embed.cu", "optim.cu", "loss.cu", "attention.cu", "comm.cu", "fp8.cu", "gemm_mx.cu"}
+PRECISE = set(CUDA_SOURCES)
 
 
 def _cuda_home() -> str:
@@ -72,7 +72,7 @@ def build_cuda(verbose: bool = True) -> str:
         if not os.path.exists(path):
             continue
         flags = [f for f in NVCC_FLAGS if not (f == "--use_fast_math" and src in PRECISE)]
-        flags += os.environ.get("B200_NVCC_EXTRA", "").split()          # e.g. -DB200_GEMM_NO_LAB for A/B builds
+        flags += os.environ.get("B200_NVCC_EXTRA", "").split()          # extra defines for A/B builds
         tag = _digest([path] + hdrs, " ".join(flags))
         obj = os.path.join(BUILD, f"{src}.{tag}.o")
         objs.append(obj)
@@ -102,7 +102,7 @@ def build_cuda(verbose: bool = True) -> str:
         f"-L{os.path.join(cuda, 'lib64')}", "-lcudart", f"-Wl,-rpath,{torch_lib}",
         f"-Wl,-rpath,{os.path.join(cuda, 'lib64')}"]
     _run(link, os.path.join(BUILD, "link.log"))
-    # objects of earlier source revisions are dead weight (hundreds of MB that every gpurun snapshot would carry)
+    # objects of earlier source revisions are dead weight (hundreds of MB)
     keep = {os.path.basename(o) for o in objs} | {os.path.basename(bind_obj)}
     for f in os.listdir(BUILD):
         if f.endswith(".o") and f not in keep:

@@ -4,7 +4,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 #include "kernels.h"
 
 namespace {
@@ -73,7 +73,7 @@ inline float* opt_f32(const c10::optional<Tensor>& t) {
 // D = epilogue(A op B).  a/b are 2-D bf16 (row stride arbitrary, multiple of 8 elements).
 //   layout 0 (NT): a [M,K], b [N,K]     1 (NN): a [M,K], b [K,N]     2 (TN): a [K,M], b [K,N]
 // fp8 mode (scale_a/scale_b given): a/b are 1-byte e4m3 (or e5m2, per flag) tensors, row strides multiples of 16,
-// scale_* are the device inv_scale floats (views into the fp8 meta table); CTA-pair kernel only.
+// scale_* are the device inv_scale floats (views into the fp8 meta table).
 static inline bool p_drop_is_zero(double p) { return !(p > 0.0); }
 
 void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::optional<Tensor> bias,
@@ -147,14 +147,14 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
   }
   TORCH_CHECK(epi != b200::EPI_BIAS_DROP_RES || c.res != nullptr, "bias+dropout+residual needs res");
   if (mask_out.has_value() && mask_out->defined()) {
-    TORCH_CHECK(epi == b200::EPI_BIAS_DROP_RES && block_n == 512 && !p_drop_is_zero(p_drop), "mask_out: dropout epilogue of the CTA-pair kernel only");
+    TORCH_CHECK(epi == b200::EPI_BIAS_DROP_RES && !p_drop_is_zero(p_drop), "mask_out: dropout epilogue only");
     TORCH_CHECK(mask_out->is_cuda() && mask_out->scalar_type() == at::kByte && mask_out->is_contiguous() &&
                 mask_out->numel() == M * (N / 8) && reinterpret_cast<uintptr_t>(mask_out->data_ptr()) % 16 == 0 && N % 128 == 0,
                 "mask_out: uint8 [M, N / 8], 16-byte aligned, N % 128 == 0");
     c.mask_out = mask_out->data_ptr<uint8_t>();
   }
   if (mask_in.has_value() && mask_in->defined()) {
-    TORCH_CHECK(epi == b200::EPI_BIAS_DROP_RES && block_n == 512 && !p_drop_is_zero(p_drop), "mask_in: dropout epilogue of the CTA-pair kernel only");
+    TORCH_CHECK(epi == b200::EPI_BIAS_DROP_RES && !p_drop_is_zero(p_drop), "mask_in: dropout epilogue only");
     TORCH_CHECK(mask_in->is_cuda() && mask_in->scalar_type() == at::kByte && mask_in->is_contiguous() &&
                 mask_in->numel() == M * (N / 8) && reinterpret_cast<uintptr_t>(mask_in->data_ptr()) % 16 == 0 && N % 128 == 0,
                 "mask_in: uint8 [M, N / 8], 16-byte aligned, N % 128 == 0");
@@ -450,37 +450,6 @@ void peer_allreduce(int64_t rank, int64_t world, bool use_multicast, std::vector
   b200::peer_allreduce(L, cur_stream());
 }
 
-// MXFP8: bf16 [R, K] -> e4m3 bytes [R, K] + ue8m0 block scales (one per 32 elements of K) in the tensor core's
-// scale-factor layout [ceil(R/128)][K/128][512]
-void mx_quantize(Tensor x, Tensor q, Tensor sf) {
-  check_bf16(x, "x");
-  TORCH_CHECK(x.dim() == 2 && x.is_contiguous() && x.size(1) % 128 == 0, "mx_quantize: contiguous [R, K] with K % 128 == 0");
-  const int64_t R = x.size(0), K = x.size(1);
-  TORCH_CHECK(q.is_cuda() && q.is_contiguous() && q.element_size() == 1 && q.numel() == R * K, "mx_quantize: q shape");
-  TORCH_CHECK(sf.is_cuda() && sf.is_contiguous() && sf.element_size() == 1 &&
-              sf.numel() == ((R + 127) / 128) * (K / 128) * 512, "mx_quantize: sf shape");
-  c10::cuda::CUDAGuard guard(x.device());
-  b200::mx_quantize(x.data_ptr(), q.data_ptr(), sf.data_ptr(), (int)R, (int)K, cur_stream());
-}
-
-// D[M,N] = A[M,K] . B[N,K]^T with block-scaled fp8 operands (tcgen05 kind::mxf8f6f4.block_scale)
-void gemm_mxfp8(Tensor a, Tensor sfa, Tensor b, Tensor sfb, Tensor out, c10::optional<Tensor> bias) {
-  TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && a.is_contiguous() && b.is_contiguous() && a.element_size() == 1 &&
-              b.element_size() == 1 && a.size(1) == b.size(1) && a.size(1) % 128 == 0, "gemm_mxfp8 operands");
-  const int64_t M = a.size(0), N = b.size(0), K = a.size(1);
-  TORCH_CHECK(sfa.numel() == ((M + 127) / 128) * (K / 128) * 512 && sfb.numel() == ((N + 127) / 128) * (K / 128) * 512,
-              "gemm_mxfp8: scale-factor sizes");
-  TORCH_CHECK(out.is_cuda() && out.dim() == 2 && out.size(0) == M && out.size(1) == N && out.stride(1) == 1 && N % 8 == 0,
-              "gemm_mxfp8: out");
-  const bool f32 = out.scalar_type() == at::kFloat;
-  TORCH_CHECK(f32 || out.scalar_type() == at::kBFloat16, "gemm_mxfp8: out must be fp32 or bf16");
-  const void* bp = nullptr;
-  if (bias.has_value() && bias->defined()) { check_bf16(*bias, "bias"); TORCH_CHECK(bias->numel() == N, "bias"); bp = bias->data_ptr(); }
-  c10::cuda::CUDAGuard guard(a.device());
-  b200::gemm_mxfp8(a.data_ptr(), sfa.data_ptr(), b.data_ptr(), sfb.data_ptr(), out.data_ptr(), (int)out.stride(0), f32, bp,
-                   (int)M, (int)N, (int)K, cur_stream());
-}
-
 void fp8_quantize(Tensor x, Tensor q, Tensor meta, bool e5m2) {
   check_bf16(x, "x");
   TORCH_CHECK(x.is_contiguous() && q.is_contiguous() && q.is_cuda() && q.element_size() == 1 && q.numel() == x.numel(),
@@ -505,16 +474,6 @@ void fp8_update(Tensor meta, Tensor is_e5m2, double margin_pow2) {
   b200::fp8_update(meta.data_ptr<float>(), (int)(meta.numel() / 4), is_e5m2.data_ptr<int>(), (float)margin_pow2, cur_stream());
 }
 
-// measurement knobs of the pair GEMM (tools/gemm_lab.py): flags as in GemmArgs::lab, stats = int64 CUDA tensor [74 * 4] or None
-void gemm_lab(int64_t flags, c10::optional<Tensor> stats) {
-  unsigned long long* sp = nullptr;
-  if (stats.has_value() && stats->defined()) {
-    TORCH_CHECK(stats->is_cuda() && stats->scalar_type() == at::kLong && stats->numel() >= 74 * 12, "gemm_lab stats");
-    sp = reinterpret_cast<unsigned long long*>(stats->data_ptr<int64_t>());
-  }
-  b200::gemm_lab((unsigned int)flags, sp);
-}
-
 // keep bits of the dropout stream (seed, stream) for a [.., N] tensor of `out.numel() * 8` elements (see dropout_mask_kernel)
 void dropout_mask(Tensor out, double p_drop, int64_t seed, int64_t stream_id) {
   TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kByte && out.is_contiguous() && out.numel() % 4 == 0 &&
@@ -527,15 +486,12 @@ void dropout_mask(Tensor out, double p_drop, int64_t seed, int64_t stream_id) {
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("dropout_mask", &dropout_mask);
-  m.def("gemm_lab", &gemm_lab);
-  m.doc() = "bert_pytorch_b200 sm_100a kernels";
+  m.doc() = "bert_pytorch_b200 sm_90a kernels";
   m.def("gemm", &gemm);
   m.def("set_seed_step", &set_seed_step);
   m.def("set_grad_peers", &set_grad_peers);
   m.def("set_grad_push", &set_grad_push);
   m.def("peer_allreduce", &peer_allreduce);
-  m.def("mx_quantize", &mx_quantize);
-  m.def("gemm_mxfp8", &gemm_mxfp8);
   m.def("fp8_quantize", &fp8_quantize);
   m.def("fp8_amax", &fp8_amax);
   m.def("fp8_update", &fp8_update);
@@ -560,6 +516,5 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("arena_adam", &arena_adam);
   m.def("attention_fwd", &attention_fwd);
   m.def("attention_bwd", &attention_bwd);
-  m.def("set_attention_options", [](int64_t bwd_pipe, int64_t row) { b200::attention_set_options((int)bwd_pipe, (int)row); });
   m.def("fused_allreduce_lamb", &fused_allreduce_lamb);
 }

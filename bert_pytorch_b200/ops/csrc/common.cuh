@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: mbarrier / TMA / tcgen05 PTX wrappers,
-// UMMA descriptor construction, Philox counter RNG for dropout, bf16 packing.
+// Shared device helpers for the sm_90a kernels: mbarrier / TMA PTX wrappers (wgmma: wgmma.cuh),
+// Philox counter RNG for dropout, bf16 packing.
 // Everything here is inline PTX written against the CUDA 12.9 ISA (no CUTLASS dependency).
 #pragma once
 #include <cuda.h>
@@ -32,7 +32,7 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 // Programmatic dependent launch (PDL): a kernel launched with launch_pdl() may become resident while its predecessor
-// in the stream is still draining; everything it does before pdl_wait() (barrier init, TMEM allocation, descriptor
+// in the stream is still draining; everything it does before pdl_wait() (barrier init, descriptor
 // prefetch) overlaps the predecessor's tail, pdl_wait() returns once the predecessor grid has completed and its
 // writes are visible.  pdl_trigger() lets the NEXT kernel's CTAs be scheduled as soon as every CTA of this grid has
 // started.  Both are no-ops for a kernel launched without the attribute.
@@ -79,8 +79,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       "selp.u32 %0, 1, 0, p;\n\t}"
       : "=r"(ok)
       : "r"(smem_u32(bar)), "r"(parity), "r"(0x4000u)   // suspend-time hint (ns): park the thread in hardware instead of
-      : "memory");                                        // spinning through the issue slots (ncu: ~20 % of the
-  return ok != 0;                                         // attention kernels' executed instructions were this loop)
+      : "memory");                                        // spinning through the issue slots
+  return ok != 0;
 }
 // Blocking wait with a watchdog: a protocol bug must trap (visible error), never hang the box.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
@@ -96,6 +96,20 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
                threadIdx.x, parity);
         __trap();
       }
+    }
+  }
+}
+
+// The same wait for threads that have wgmma groups in flight: no printf (a function call inside the wgmma pipeline
+// makes ptxas serialise the MMAs), the watchdog only traps.
+__device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
+  uint64_t t0 = 0;
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++spins & 255u) == 0) {
+      const uint64_t now = globaltimer_ns();
+      if (t0 == 0) t0 = now;
+      if (now - t0 > B200_WATCHDOG_NS) __trap();
     }
   }
 }
@@ -147,202 +161,6 @@ __device__ __forceinline__ void tma_store_wait_read() {
 template <int N>
 __device__ __forceinline__ void tma_store_wait() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, load
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], bf16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (bf16 packed), B from smem.
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// wait::ld that names the destination registers, so that no use of them can be scheduled above the wait when several
-// loads are kept in flight across other work (software-pipelined epilogues)
-__device__ __forceinline__ void tmem_ld_wait_dep(uint32_t (&v)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]),
-                 "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]),
-                 "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait_dep16(uint32_t (&v)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15])
-               :: "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets row (lane base + t), v[j] = column j.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-// store 16 packed 32-bit words per lane (used to place bf16 P tiles into TMEM as an MMA A operand)
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-      "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-      "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two SMs of one TPC run one 256-row UMMA; launched as a 2-CTA cluster
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of `local_smem_addr`'s twin in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load issued by either CTA of a pair; the completion bytes are credited to the barrier at
-// `mbar_cluster_addr` (the leader CTA's barrier)
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint32_t mbar_cluster_addr,
-                                                int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(void* smem_dst, const CUtensorMap* m, uint32_t mbar_cluster_addr,
-                                                int32_t c0, int32_t c1, int32_t c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster_addr), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem, uint32_t ncols) {  // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// fp8 operands (e4m3 / e5m2 selected in the instruction descriptor), fp32 accumulation: K = 32 per instruction
-__device__ __forceinline__ void umma_fp8_ss_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once the issued MMAs retire) on the barrier at the same offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// UMMA descriptors (layout per cute/arch/mma_sm100_desc.hpp: SmemDescriptor / InstrDescriptor)
-// ------------------------------------------------------------------------------------------------
-// 64-bit shared-memory matrix descriptor, 128-byte swizzle, Blackwell version field = 1.
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version (1)   bits [61,64) layout (2 = SWIZZLE_128B)
-__host__ __device__ constexpr uint64_t umma_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                            uint32_t sbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// 32-bit instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D fmt (1=f32)  [7,10) A fmt (1=bf16)  [10,13) B fmt (1=bf16)  [15] A major (1=MN)  [16] B major
-//   [17,23) N>>3   [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// kind::f8f6f4: same field layout; A/B format 0 = e4m3, 1 = e5m2
-__host__ __device__ constexpr uint32_t umma_idesc_fp8(uint32_t M, uint32_t N, bool a_mn_major, bool b_mn_major,
-                                                      uint32_t a_e5m2, uint32_t b_e5m2) {
-  return (1u << 4) | ((a_e5m2 & 1u) << 7) | ((b_e5m2 & 1u) << 10) | ((a_mn_major ? 1u : 0u) << 15) |
-         ((b_mn_major ? 1u : 0u) << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -478,51 +296,22 @@ __device__ __forceinline__ float dgelu_erf(float x) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Packed fp32 pairs (sm_100: FFMA2 / FMUL2 / FADD2 issue one instruction for two lanes of fp32 math).  The GEMM
-// epilogues are issue bound (K = 1024: the tensor cores finish one output element per SMSP and clock, i.e. 32
-// warp-instructions per element is ALL there is), so every FMA-class operation of the epilogue math runs two wide.
+// fp32 pairs: two independent lanes of fp32 math behind one name (sm_90 has no packed fp32 instructions; each
+// operation is two scalar FFMA / FMUL / FADD with the same rounding as the scalar code).
 // ------------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_pack_u(uint32_t lo, uint32_t hi) {
-  f32x2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ float2 f2_unpack(f32x2 v) {
-  float2 r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_splat(float c) { return f2_pack(c, c); }
-__device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) {
-  f32x2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) {
-  f32x2 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
+struct f32x2 { float x, y; };
+__device__ __forceinline__ f32x2 f2_pack(float lo, float hi) { return f32x2{lo, hi}; }
+__device__ __forceinline__ f32x2 f2_pack_u(uint32_t lo, uint32_t hi) { return f32x2{__uint_as_float(lo), __uint_as_float(hi)}; }
+__device__ __forceinline__ float2 f2_unpack(f32x2 v) { return make_float2(v.x, v.y); }
+__device__ __forceinline__ f32x2 f2_splat(float c) { return f32x2{c, c}; }
+__device__ __forceinline__ f32x2 f2_fma(f32x2 a, f32x2 b, f32x2 c) { return f32x2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
+__device__ __forceinline__ f32x2 f2_mul(f32x2 a, f32x2 b) { return f32x2{a.x * b.x, a.y * b.y}; }
+__device__ __forceinline__ f32x2 f2_add(f32x2 a, f32x2 b) { return f32x2{a.x + b.x, a.y + b.y}; }
 __device__ __forceinline__ f32x2 f2_from_bf16x2(uint32_t w) {       // {lo, hi} bf16 -> two fp32 (exact)
   return f2_pack_u(w << 16, w & 0xffff0000u);
 }
-__device__ __forceinline__ uint32_t f2_to_bf16x2(f32x2 v) {
-  const float2 f = f2_unpack(v);
-  return pack_bf16(f.x, f.y);
-}
-// gelu(x) and gelu'(x) of two values: the same arithmetic as gelu_parts(), FMA-class work two wide
-// (26 instructions per PAIR: 4 MUFU, 2 FFMA with |x|, 4 select, 2 pack, 14 packed -- 28 per element before)
+__device__ __forceinline__ uint32_t f2_to_bf16x2(f32x2 v) { return pack_bf16(v.x, v.y); }
+// gelu(x) and gelu'(x) of two values: the same arithmetic as gelu_parts()
 struct GeluDg2 { f32x2 g, dg; };
 __device__ __forceinline__ GeluDg2 gelu_dg2(f32x2 x) {
   const float2 xf = f2_unpack(x);
@@ -597,6 +386,18 @@ __device__ __forceinline__ void fp8_amax_commit(const Fp8Out& f, float amax) {
       abort();                                                                                  \
     }                                                                                           \
   } while (0)
+
+namespace b200 {
+inline int num_sms() {                   // SMs of the current device (132 on an H100 SXM)
+  static int n = 0;
+  if (n == 0) {
+    int dev;
+    B200_CUDA_CHECK(cudaGetDevice(&dev));
+    B200_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+  }
+  return n;
+}
+}  // namespace b200
 
 // launch with the programmatic-stream-serialization attribute (see pdl_wait above); B200_PDL=0 launches plainly
 #include <utility>

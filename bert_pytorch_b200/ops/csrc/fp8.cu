@@ -1,6 +1,6 @@
-// Per-tensor scaled fp8 (e4m3 / e5m2) operand preparation for the tcgen05 kind::f8f6f4 GEMM path.
+// Per-tensor scaled fp8 (e4m3 / e5m2) operand preparation for the wgmma fp8 GEMM path.
 //
-// Recipe (delayed scaling; the reference has no fp8 path -- BASELINE.json's RoBERTa fp8 config is a B200 addition):
+// Recipe (delayed scaling; the reference has no fp8 path -- BASELINE.json's RoBERTa fp8 config is an addition of this project):
 //   every GEMM operand site owns a 4-float record  meta = {amax, scale, inv_scale, _}  on the device
 //   quantise:     q = sat_fp8(x * scale)      and   amax = max(amax, |x|)      (one pass over x, 3 B/element)
 //   GEMM:         D = (qa . qb) * inv_scale_a * inv_scale_b                     (read by the epilogue from meta)
@@ -87,7 +87,7 @@ __global__ void fp8_update_kernel(float* __restrict__ meta, int nrec, const int*
 void fp8_quantize(const void* x, void* q, long long n, float* meta, bool e5m2, cudaStream_t st) {
   const long long n16 = n / 16;
   if (n16 == 0) return;
-  const int grid = (int)std::min<long long>((n16 + 255) / 256, 148 * 8);
+  const int grid = (int)std::min<long long>((n16 + 255) / 256, num_sms() * 8);
   if (e5m2) fp8_quantize_kernel<true><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (uint8_t*)q, n16, meta);
   else fp8_quantize_kernel<false><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (uint8_t*)q, n16, meta);
 }
@@ -95,7 +95,7 @@ void fp8_quantize(const void* x, void* q, long long n, float* meta, bool e5m2, c
 void fp8_amax(const void* x, long long n, float* meta, cudaStream_t st) {
   const long long n8 = n / 8;
   if (n8 == 0) return;
-  const int grid = (int)std::min<long long>((n8 + 255) / 256, 148 * 8);
+  const int grid = (int)std::min<long long>((n8 + 255) / 256, num_sms() * 8);
   fp8_amax_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, n8, meta);
 }
 

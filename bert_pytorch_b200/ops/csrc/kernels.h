@@ -50,10 +50,9 @@ void arena_adam(float* g, float* p, float* m, float* v, void* shadow, const int*
                 const float* inv_scale, const float* found_inf, float lr, float beta1, float beta2, float eps,
                 float weight_decay, int step, int bias_correction, int adam_w_mode, cudaStream_t st);
 
-// attention.cu
+// attention_sm90.cu
 void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, int B, int S, int h, int d,
                    float scale, Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st);
-void attention_set_options(int bwd_pipe, int row_kernels);   // each: -1 env default, 0 / 1 force off / on
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
                    Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st);
@@ -92,11 +91,6 @@ void peer_allreduce(const PeerAllreduceLaunch& L, cudaStream_t st);
 // loss.cu: NSP classifier + CE + backward in one launch
 void nsp_head(const void* pooled_bf16, const void* w_bf16, const float* bias, const long long* labels, int B, int H,
               float grad_scale, float* loss_out, void* dz_bf16, float* dw, float* db, cudaStream_t st);
-
-// gemm_mx.cu: block-scaled MXFP8 (e4m3 + one ue8m0 scale per 32 elements along K), NT layout
-void mx_quantize(const void* x_bf16, void* q, void* sf, int R, int K, cudaStream_t st);
-void gemm_mxfp8(const void* a, const void* sfa, const void* b, const void* sfb, void* out, int ldo, bool out_f32,
-                const void* bias, int M, int N, int K, cudaStream_t st);
 
 // fp8.cu: per-tensor scaled fp8 operand preparation; meta records are {amax, scale, inv_scale, _}
 void fp8_quantize(const void* x_bf16, void* q, long long n, float* meta, bool e5m2, cudaStream_t st);

@@ -393,9 +393,8 @@ ln_bwd2_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
 }
 
 // ------------------------------------------------------------------------------------------------
-// Round-2 fast paths (H == CHUNKS * 256, no fp8 side output).  ncu on the kernels above: ~60 % issue-slot
-// utilisation at 15-22 % DRAM throughput -- they are instruction bound (per-row reductions, barriers and address
-// arithmetic amortised over only 8 elements per lane), so these variants cut instructions per element:
+// Fast paths (H == CHUNKS * 256, no fp8 side output).  The kernels above are instruction bound (per-row reductions,
+// barriers and address arithmetic amortised over only 8 elements per lane), so these variants cut instructions per element:
 //   forward : one warp owns a whole row (32 elements per lane): shuffle-only statistics, exact two-pass variance in
 //             registers, gamma / beta from shared memory (conflict-free float4 layout); ~8 instructions per element
 //   backward: same lane-owns-8-columns layout as ln_bwd2 (the column sums for dgamma / dbeta / dbias must stay in
@@ -469,10 +468,9 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
                __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dxd, float* __restrict__ partial, int M,
                Seed seed_in, unsigned int drop_stream, unsigned int thresh16, float drop_scale,
                const uint8_t* __restrict__ keep_mask) {
-  // Round 2b: (1) all FMA-class work on packed fp32 pairs (FFMA2 / FMUL2 / FADD2: the kernel is issue bound -- 290
-  // instructions per 8-element slice before), (2) the dropout decisions of the residual branch are READ (one byte per
-  // 8 elements, written by the producing GEMM epilogue: GemmCall::mask_out) instead of regenerated with Philox
-  // (60 of the 290) whenever the caller has them.
+  // The dropout decisions of the residual branch are READ (one byte per 8 elements, written by dropout_mask_kernel
+  // or by the producing GEMM epilogue: GemmCall::mask_out) instead of regenerated with Philox whenever the caller
+  // has them.
   constexpr int H = WPR * 256;
   __shared__ float2 xchg[GROUPS][2][WPR];
   __shared__ float comb[GROUPS - 1 > 0 ? GROUPS - 1 : 1][3][H];
@@ -489,7 +487,7 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
     g2[0] = f2_pack(g0.x, g0.y); g2[1] = f2_pack(g0.z, g0.w); g2[2] = f2_pack(g1.x, g1.y); g2[3] = f2_pack(g1.z, g1.w);
   }
 #pragma unroll
-  for (int t = 0; t < 4; ++t) ag2[t] = ab2[t] = ad2[t] = 0ull;
+  for (int t = 0; t < 4; ++t) ag2[t] = ab2[t] = ad2[t] = f2_splat(0.f);
   const int stride = gridDim.x * GROUPS;
   int row = blockIdx.x * GROUPS + group;
   uint4 nd = make_uint4(0, 0, 0, 0), nv = make_uint4(0, 0, 0, 0);
@@ -517,7 +515,7 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
       if (use_mask) nmask = __ldg(keep_mask + (size_t)nrow * (H / 8) + (col >> 3));
     }
     const f32x2 rs2 = f2_splat(rs), nmr2 = f2_splat(nmr);
-    f32x2 xh[4], dg[4], s1p = 0ull, s2p = 0ull;
+    f32x2 xh[4], dg[4], s1p = f2_splat(0.f), s2p = f2_splat(0.f);
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
       const f32x2 d = f2_from_bf16x2(dw[t]);
@@ -845,8 +843,8 @@ embed_bwd_scatter_kernel(const __nv_bfloat16* __restrict__ de, const int* __rest
   }
 }
 
-// Position / token-type gradients as REDUCTIONS instead of atomics (ncu round 2: the scatter kernel spent 269 us in
-// lg_throttle -- 12288 rows hammering the two token-type rows and 96 rows per position row).  Thread (s, 8 columns)
+// Position / token-type gradients as REDUCTIONS instead of atomics (12288 rows hammering the two token-type rows and
+// 96 rows per position row serialise in L2).  Thread (s, 8 columns)
 // walks the batch dimension: the position row s has exactly one owner (plain read-modify-write), the two token-type
 // rows are reduced over the 8 positions of a block in shared memory and leave as one atomic per block and column.
 __global__ void __launch_bounds__(256)
@@ -959,7 +957,7 @@ static inline void drop_params(float p, unsigned int& thresh, float& scale) {
 }
 static inline int ln_grid(int M) {
   int g = (M + LN_WARPS - 1) / LN_WARPS;
-  return g < 148 * 8 ? g : 148 * 8;
+  return g < num_sms() * 8 ? g : num_sms() * 8;
 }
 
 #define DISPATCH_CHUNKS(H, ...)                                    \
@@ -986,7 +984,7 @@ static inline int ln_grid(int M) {
 
 static inline int ln2_grid(int M) {     // 2 rows per block at a time; 4 resident blocks per SM
   int g = (M + 1) / 2;
-  return g < 148 * 4 ? g : 148 * 4;
+  return g < num_sms() * 4 ? g : num_sms() * 4;
 }
 
 static bool ln_fast_enabled() {
@@ -1000,7 +998,7 @@ void layer_norm_fwd(const void* x, const float* gamma, const float* beta, void* 
   drop_params(p_drop, th, sc);
   if (ln_fast_enabled() && th == 0 && f8.q == nullptr && H % 256 == 0 && H <= 1024) {   // warp-per-row fast path
     int g = (M + 7) / 8;
-    if (g > 148 * 4) g = 148 * 4;
+    if (g > num_sms() * 4) g = num_sms() * 4;
     const __nv_bfloat16* xp = (const __nv_bfloat16*)x;
     __nv_bfloat16* yp = (__nv_bfloat16*)y;
     switch (H / 256) {
@@ -1014,7 +1012,7 @@ void layer_norm_fwd(const void* x, const float* gamma, const float* beta, void* 
   static const bool two_rows = []() { const char* e = getenv("B200_LN_ROWS"); return e && e[0] == '2'; }();
   if (two_rows) {                        // measured slower than one row (24.6 vs 22.6 us): kept for reference only
     int g4 = (M + 3) / 4;
-    if (g4 > 148 * 3) g4 = 148 * 3;
+    if (g4 > num_sms() * 3) g4 = num_sms() * 3;
     DISPATCH_WPR(H, (ln_fwd2x2_kernel<WPR><<<g4, 2 * WPR * 32, 0, st>>>(
         (const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, M, H, eps, seed, stream, th, sc, f8)));
     return;
@@ -1027,7 +1025,7 @@ void layer_norm_fwd(const void* x, const float* gamma, const float* beta, void* 
 // ran a 1/3-full second wave)
 static inline int ln2_bwd_grid(int M) {
   int g = (M + 1) / 2;
-  return g < 148 * 3 ? g : 148 * 3;
+  return g < num_sms() * 3 ? g : num_sms() * 3;
 }
 
 int ln_bwd_workspace_floats(int M, int H) { return ln2_grid(M) * 3 * H; }
@@ -1040,7 +1038,7 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
   drop_params(p_drop, th, sc);
   static const int split = []() {
     const char* e = getenv("B200_LN_FINALIZE_SPLIT");
-    const int z = e ? atoi(e) : 8;       // 8 slices: 39.9 vs 44.0 us for the pair of launches (elt_bench, round 2)
+    const int z = e ? atoi(e) : 8;
     return z < 1 ? 1 : (z > 32 ? 32 : z);
   }();
   if (ln_fast_enabled() && f8.q == nullptr && (in_stream == 0xFFFFFFFFu || th == 0) && H % 256 == 0 && H <= 1024) {
@@ -1071,9 +1069,8 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
 
 // Keep bits of one hidden-dropout site, one byte per 8 elements ([M][N / 8], bit t of byte j = element 8 j + t kept):
 // the same decisions as dropout_keep8(seed, stream, e8) with e8 = (row * N + col) / 8.  Generated here, with every warp
-// of the machine busy, instead of inside the GEMM epilogue that applies them (two epilogue warps per SMSP: the Philox
-// rounds were 9.6 k of the 13.6 k cycles the dropout + residual epilogue spent per tile -- gemm_lab phase clock -- against
-// 8.2 k cycles of MMAs per K = 1024 tile) and instead of being regenerated by the LayerNorm backward.
+// of the machine busy, instead of inside the GEMM epilogue that applies them (where the tensor cores idle
+// meanwhile) and instead of being regenerated by the LayerNorm backward.
 __global__ void __launch_bounds__(256) dropout_mask_kernel(unsigned int* __restrict__ out, long long n_words, Seed seed_in,
                                                            unsigned int stream, unsigned int thresh16) {
   pdl_trigger_small();
@@ -1096,7 +1093,7 @@ void dropout_mask(void* out, long long n_elems, Seed seed, unsigned int stream, 
   drop_params(p_drop, th, sc);
   const long long n_words = n_elems / 32;
   long long g = (n_words + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > num_sms() * 16) g = num_sms() * 16;
   if (g > 0) launch_pdl(dropout_mask_kernel, dim3((unsigned)g), dim3(256), 0, st, (unsigned int*)out, n_words, seed, stream, th);
 }
 
@@ -1108,7 +1105,7 @@ void colsum_bf16(const void* x, int M, int N, int ld, float* out, cudaStream_t s
 void gelu_fwd(const void* x, void* y, long long n, Fp8Out f8, cudaStream_t st) {
   const long long n8 = n >> 3;
   long long g = (n8 + 255) / 256;
-  if (g > 148 * 32) g = 148 * 32;
+  if (g > num_sms() * 32) g = num_sms() * 32;
   if (g > 0) gelu_fwd_kernel<<<(unsigned)g, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, n8, f8);
 }
 void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int N, Fp8Out f8, cudaStream_t st) {
@@ -1130,7 +1127,7 @@ void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float
                            int M, int S, int H, int type_rows, cudaStream_t st) {
   const size_t work = (size_t)M * (H / 8);
   int grid = (int)((work + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > num_sms() * 16) grid = num_sms() * 16;
   static const bool reduce_ok = []() { const char* e = getenv("B200_EMBED_REDUCE"); return !(e && e[0] == '0'); }();
   if (reduce_ok && M % S == 0 && H % 8 == 0 && (gtype == nullptr || type_rows == 2)) {
     // word rows: scatter with atomics (30 k rows, little contention); position / token-type rows: reductions
@@ -1150,13 +1147,13 @@ void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* t
 void gather_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st) {
   const size_t work = (size_t)n * (H / 8);
   int grid = (int)((work + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > num_sms() * 16) grid = num_sms() * 16;
   if (grid > 0) gather_rows_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)src, idx, (__nv_bfloat16*)dst, n, H);
 }
 void scatter_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st) {
   const size_t work = (size_t)n * (H / 8);
   int grid = (int)((work + 255) / 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > num_sms() * 16) grid = num_sms() * 16;
   if (grid > 0) scatter_rows_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)src, idx, (__nv_bfloat16*)dst, n, H);
 }
 

@@ -295,10 +295,10 @@ void mt_scale(int in_dtype, int out_dtype, const long long* in_ptrs, const long 
 
 void flat_sumsq(const float* g, long long n, const float* inv_scale, float* stats, float* found_inf, cudaStream_t st) {
   B200_CUDA_CHECK(cudaMemsetAsync(stats, 0, sizeof(float), st));
-  flat_sumsq_kernel<<<148 * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, stats, found_inf);
+  flat_sumsq_kernel<<<num_sms() * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, stats, found_inf);
 }
 void flat_unscale(float* g, long long n, const float* inv_scale, float* found_inf, cudaStream_t st) {
-  flat_unscale_kernel<<<148 * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, found_inf);
+  flat_unscale_kernel<<<num_sms() * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, found_inf);
 }
 
 void arena_lamb(float* g, float* p, float* m, float* v, void* shadow, const int* chunk_tensor,

@@ -2,7 +2,7 @@
 
 * :class:`Adam` -- contract of apex ``FusedAdam`` (AdamW-style decoupled decay,
   optional bias correction; both reference call sites pass ``bias_correction=False``:
-  run_squad.py:982-988, run_ner.py:243-244).  Fused multi-tensor sm_100a kernel when the
+  run_squad.py:982-988, run_ner.py:243-244).  Fused multi-tensor sm_90a kernel when the
   parameters live in a ParamArena, pure torch otherwise.
 * :class:`BertAdam` -- src/optimization.py:64-174: Adam without bias correction,
   decoupled decay, per-parameter gradient clipping and a built-in warm-up schedule

@@ -9,7 +9,7 @@
 
 Two execution paths share this class:
   * the pure-torch path below (CPU, gloo runs, and the numerics oracle for tests);
-  * the sm_100a multi-tensor kernels (ops/csrc/optim.cu) when the parameters live in a
+  * the sm_90a multi-tensor kernels (ops/csrc/optim.cu) when the parameters live in a
     :class:`~bert_pytorch_b200.models.arena.ParamArena` on a CUDA device -- one pass
     for the global grad norm (+ unscale + inf/nan flag), one for moments/update/
     per-tensor norms, one for the trust-ratio apply that also refreshes the bf16

@@ -7,7 +7,7 @@
   barriers).  Lets the partitioned all-reduce+LAMB *algorithm* (shard bounds, two-phase
   norms, inf-skip agreement) be verified bit-for-bit on a box with no GPU and no network.
 * :class:`bert_pytorch_b200.parallel.peer.PeerComm` -- the product path: CUDA peer memory
-  (symmetric buffers mapped into every rank) driven by our own sm_100a kernels; no NCCL on
+  (symmetric buffers mapped into every rank) driven by our own sm_90a kernels; no NCCL on
   the gradient path.
 
 Every backend offers: all_reduce_ (sum / avg / max), reduce_scatter (contiguous shards),

@@ -8,7 +8,7 @@ Semantics kept:
     micro-steps inside ``no_sync()`` only accumulate locally (X4);
   * ``module`` attribute / ``state_dict`` of the wrapped model are untouched.
 
-Differences (B200-first): gradients already live in one flat fp32 arena
+Differences (H100-first): gradients already live in one flat fp32 arena
 (:class:`~bert_pytorch_b200.models.arena.ParamArena`), so there is no bucket copy-in /
 copy-out -- the reduction runs in place over ``bucket_bytes`` slices of the arena, launched on
 a side stream so the tail of backward overlaps it.  With ``backend='fused'`` the reduction is

@@ -6,7 +6,7 @@ fabric offers it) and replaces
 
     DDP bucketed ncclAllReduce  ->  GradScaler.unscale_  ->  FusedLAMB  (reference: run_pretraining.py:405-458)
 
-by ONE persistent sm_100a kernel per optimizer step (ops/csrc/comm.cu): reduce-scatter of the gradient
+by ONE persistent sm_90a kernel per optimizer step (ops/csrc/comm.cu): reduce-scatter of the gradient
 shards with P2P loads / ``multimem.ld_reduce``, fused 1/(world*scale) + inf/nan detection, partitioned LAMB
 with cross-rank norm exchange through peer stores, and the parameter all-gather as P2P / ``multimem.st``
 stores of the updated fp32 + bf16 values.  No NCCL call on this path.  The bootstrap (rendezvous, handle
@@ -46,8 +46,8 @@ class PeerComm(TorchComm):
         super().__init__(group)
         import os
         # push_master=False keeps the fp32 master weights shard-local (ZeRO-1 style): only the bf16 weights the
-        # kernels read (and the fp32 1-D tensors) are all-gathered, 3x less NVLink traffic: 3.2 vs 5.0 ms per step
-        # at 8 GPUs (profiles/peer_check_r1_8gpu.log).  ``gather_master()`` completes the fp32 views before
+        # kernels read (and the fp32 1-D tensors) are all-gathered, 3x less NVLink traffic.
+        # ``gather_master()`` completes the fp32 views before
         # anything reads them (checkpoint, ``arena.refresh_shadow``, torch-path evaluation).  The pre-training
         # runtime selects it (pretrain.configure_fused_reduction); B200_PEER_MASTER_LOCAL=0/1 overrides.
         if push_master is None:
@@ -94,8 +94,7 @@ class PeerComm(TorchComm):
         self.arena = arena
         arena._master_sync = self.gather_master
         mc_ok = all(int(getattr(h, "multicast_ptr", 0) or 0) != 0 for h in (self.grad_h, self.param_h))
-        # NVLS multimem wins from 4 ranks up (in-switch reduction / replication); at 2 ranks plain P2P is faster
-        # (measured: profiles/peer_check_r1_2gpu_v3.log, peer_check_r1_8gpu.log)
+        # NVLS multimem from 4 ranks up (in-switch reduction / replication); plain P2P at 2 ranks
         self.use_multicast = (mc_ok and self.world_size > 2) if self._want_mc is None else (bool(self._want_mc) and mc_ok)
         self.lo, self.hi = arena.shard_bounds(self.world_size, self.rank, GRANULE)
         # chunk table of the arena restricted to the shard
@@ -313,7 +312,7 @@ class HierarchicalPeerComm(TorchComm):
     the same parameters and (partitioned) LAMB state, so checkpoints gather inside node 0 only.
     Generic collectives (broadcast at start-up, K-FAC factors, barriers) use the world NCCL group.
     The rail all-reduce moves the whole arena; shard-only traffic needs the reduction kernel split at the phase
-    boundary (NOTES.md)."""
+    boundary."""
     fuses_optimizer = True
 
     def __init__(self, local_world: int, **peer_kw):

@@ -1,6 +1,6 @@
 """Partitioned ("ZeRO-1 style") LAMB fused with the gradient reduction -- the *algorithm*,
 written against the :class:`Comm` interface so it runs on gloo / the in-process fake and is
-the executable specification for the sm_100a peer-memory kernel (ops/csrc/comm.cu;
+the executable specification for the sm_90a peer-memory kernel (ops/csrc/comm.cu;
 SURVEY.md 5.8 items 3-4, 7.5 hard part #3).
 
 Per optimizer step, on a flat gradient arena of ``numel`` elements split into one

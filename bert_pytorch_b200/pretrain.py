@@ -5,7 +5,7 @@ and metric logging.  ``run_pretraining.py`` at the repo root is the CLI shim.
 Function names, flags, output files and checkpoint layout follow the reference
 (run_pretraining.py:75-600; SURVEY.md 2.5.1/2.5.2/5.4); the execution underneath does not:
   * parameters/gradients/moments live in a flat arena; on CUDA the forward/backward of the
-    whole model is the fused sm_100a engine (models/fused.py) and the optimizer step is the
+    whole model is the fused sm_90a engine (models/fused.py) and the optimizer step is the
     multi-tensor LAMB kernels; on CPU everything runs the plain-PyTorch oracle path;
   * ``--backend fused`` replaces DDP's NCCL all-reduce + unscale + LAMB by one peer-memory
     kernel sequence (parallel/peer.py); ``nccl`` / ``gloo`` remain (baseline / CPU plumbing);
@@ -51,7 +51,7 @@ from .utils.timing import DeviceTimer, StepClock, max_over_ranks, nvtx_range
 # ---------------------------------------------------------------------------
 
 def build_parser() -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description="BERT pre-training (B200-native)")
+    p = argparse.ArgumentParser(description="BERT pre-training (H100-native)")
     p.add_argument("--config_file", default=None, type=str, help="JSON config overriding the defaults below")
     # required (may come from the JSON)
     p.add_argument("--input_dir", default=None, type=str, help="file or directory (recursive *.hdf5)")
@@ -68,7 +68,7 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--log_prefix", type=str, default="logfile")
     p.add_argument("--seed", type=int, default=42)
     p.add_argument("--fp16", default=False, action="store_true",
-                   help="reference flag: dynamic loss scaling (GradScaler) on. On a B200 the fused engine multiplies bf16 "
+                   help="reference flag: dynamic loss scaling (GradScaler) on. On an H100 the fused engine multiplies bf16 "
                         "operands either way -- fp16 selects the scaler semantics, not fp16 tensor-core operands "
                         "(DESIGN.md section 2); the plain-PyTorch fallback path autocasts to fp16")
     # hyper-parameters
@@ -96,7 +96,7 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--device", default=None, choices=[None, "cuda", "cpu"])
     p.add_argument("--no_fused", default=False, action="store_true", help="run the plain-PyTorch oracle path")
     p.add_argument("--fp8", default=False, action="store_true",
-                   help="B200 extension: fp8 GEMM operands in the fused engine (e4m3 activations/weights, e5m2 gradients, "
+                   help="fp8 GEMM operands in the fused engine (e4m3 activations/weights, e5m2 gradients, "
                         "per-tensor delayed scaling); LayerNorm, attention, master weights unchanged")
     p.add_argument("--loader_depth", type=int, default=4)
     return p
@@ -336,7 +336,7 @@ def forward_backward_pass(model, criterion, scaler, batch, divisor, sync_grads=T
     engine = base.pretrain_engine() if hasattr(base, "pretrain_engine") else None
     loss_scale = scaler.get_scale() if (scaler is not None and scaler.is_enabled()) else 1.0
     if engine is not None:
-        # fused sm_100a path: forward + backward in one call, grads accumulate into the arena
+        # fused sm_90a path: forward + backward in one call, grads accumulate into the arena
         comm = getattr(model, "comm", None)
         kf = getattr(base.bert, "_kfac", None) if hasattr(base, "bert") else None
         if kf is not None:                   # K-FAC statistics only where they count; all other micro-steps replay the graph

@@ -1,6 +1,6 @@
 """Host-side (numpy) evaluation of the kernels' dropout masks.
 
-Every dropout site of the sm_100a kernels draws its keep decisions from Philox4x32-7 keyed by ``seed`` with the
+Every dropout site of the sm_90a kernels draws its keep decisions from Philox4x32-7 keyed by ``seed`` with the
 counter ``(element_index >> 3, stream, 0x5EED)`` -- 128 random bits per group of 8 consecutive elements, 16 bits per
 element, kept iff ``bits >= round(p * 65536)`` (ops/csrc/common.cuh: ``Philox::gen`` / ``dropout_keep8`` / ``philox7``).
 Reproducing that here lets a test feed the SAME masks to an fp32 autograd oracle and compare gradients tensor by

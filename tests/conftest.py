@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (runs on the B200 box only)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (needs an H100)")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 CUDA devices")
 
 

@@ -41,13 +41,15 @@ def test_build_script_lists_every_cuda_source():
 
 
 def test_tile_variant_heuristic_sends_the_bert_large_shapes_to_the_cta_pair_kernel():
-    """ops.api.pick_block_n: every GEMM of a BERT-large layer (and the vocabulary projection) runs on the 2-CTA
-    256 x 256 kernel; the fine-tuning heads (N padded to 8) and one-row-block problems fall back to single-CTA tiles."""
+    """(The name dates from a 2-CTA kernel; the wide variant is the 128 x 256 tile now.)
+    ops.api.pick_block_n: every GEMM of a BERT-large layer (and the vocabulary projection) runs on 128 x 256 tiles;
+    the fine-tuning heads (N padded to 8) run on 128 x 128 tiles, one-row-block problems on whichever fills more SMs."""
     from bert_pytorch_b200.ops import api
-    for M, N in ((12288, 1024), (12288, 3072), (12288, 4096), (1920, 30528), (8192, 1024), (1024, 1024), (4096, 1024)):
-        assert api.pick_block_n(M, N) == 512, (M, N)
+    for M, N in ((12288, 1024), (12288, 3072), (12288, 4096), (1920, 30528), (8192, 1024), (4096, 1024)):
+        assert api.pick_block_n(M, N) == 256, (M, N)
     assert api.pick_block_n(12288, 8) == 128            # QA / token-classification heads
     assert api.pick_block_n(96, 1024) in (128, 256)     # pooler: one 128-row block, whichever fills more SMs
     assert api.pick_block_n(128, 4096) in (128, 256)
+    assert api.pick_block_n(1024, 1024) in (128, 256)
     # the narrow variant only when it wastes (clearly) fewer SM slots in the last wave
-    assert api._pick_block_n(128, 148 * 128) == 128 or not api._PAIR_ENABLED
+    assert api._pick_block_n(128, api.NUM_SMS * 128) == 128

@@ -1,4 +1,4 @@
-"""tcgen05 fused attention (forward + backward) vs an fp32 PyTorch reference of the same op."""
+"""wgmma fused attention (forward + backward) vs an fp32 PyTorch reference of the same op."""
 import math
 
 import pytest
@@ -54,7 +54,7 @@ def test_attention_fwd_bwd_no_dropout(B, S, heads, lens):
     assert err < 4e-2 * max(scale, 1.0), (err, scale)
 
 
-@pytest.mark.parametrize("S", [256, 128])          # 128: the single-block kernels (two / three CTAs per SM)
+@pytest.mark.parametrize("S", [256, 128])          # 128: one key block
 def test_attention_dropout_statistics_and_adjoint(S):
     K = _api()
     torch.manual_seed(0)
@@ -86,42 +86,16 @@ def test_attention_dropout_statistics_and_adjoint(S):
     assert abs(rhs2 - rhs) > 1e-3 * max(abs(rhs), 1.0)
 
 
-@pytest.mark.skipif(__import__("os").environ.get("B200_TEST_EXPERIMENTAL") != "1",
-                    reason="opt-in kernels that have not been measured on a B200 yet (B200_TEST_EXPERIMENTAL=1)")
-@pytest.mark.parametrize("B,S,heads,lens,p_drop", [
-    (2, 512, 2, [512, 300], 0.0), (2, 256, 2, [256, 130], 0.0), (2, 384, 2, [384, 129], 0.0), (3, 512, 4, [512, 1, 200], 0.1),
-])
-def test_pipelined_streaming_backward_matches_serial_kernel(B, S, heads, lens, p_drop):
-    """The software-pipelined S > 128 backward (attn_bwd_pipe_kernel) against the serial streaming kernel: same
-    inputs, same dropout stream -> the same dQ/dK/dV up to the fp32 atomics order of dQ."""
-    K = _api()
-    torch.manual_seed(1)
-    H = heads * 64
-    qkv = (torch.randn(B, S, 3 * H, device="cuda") * 0.7).to(torch.bfloat16)
-    seqlens = torch.tensor(lens, device="cuda", dtype=torch.int32)
-    ctx, lse = K.attention_fwd(qkv, seqlens, heads, p_drop=p_drop, seed=77, stream=5)
-    dctx = (torch.randn(B, S, H, device="cuda") * 0.5).to(torch.bfloat16)
-    try:
-        K.set_attention_options(bwd_pipe=False)
-        ref = K.attention_bwd(qkv, seqlens, ctx, dctx, lse, heads, p_drop=p_drop, seed=77, stream=5).float()
-        K.set_attention_options(bwd_pipe=True)
-        for _ in range(3):                       # repeat: races show up as run-to-run differences
-            out = K.attention_bwd(qkv, seqlens, ctx, dctx, lse, heads, p_drop=p_drop, seed=77, stream=5).float()
-            torch.cuda.synchronize()
-            scale = ref.abs().max().item()
-            assert (out - ref).abs().max().item() <= 1e-2 * max(scale, 1.0)
-    finally:
-        K.set_attention_options(None, None)
-
-
 @pytest.mark.parametrize("B,S,heads,lens,p_drop", [
     (3, 128, 4, [128, 77, 1], 0.1), (2, 128, 2, [128, 64], 0.0), (2, 64, 2, [64, 50], 0.1),
     (3, 512, 4, [512, 300, 129], 0.1), (2, 256, 2, [256, 130], 0.1), (2, 384, 2, [384, 1], 0.0), (40, 128, 16, None, 0.1),
 ])
 def test_row_kernels_match_round1_kernels(B, S, heads, lens, p_drop):
-    """The thread-per-row / persistent kernels of round 2 against the two-threads-per-row kernels of round 1 on the
-    same inputs and the same dropout stream: same Philox bits, so context, log-sum-exp and all three gradients must
-    agree to bf16 rounding (the big case has more items than resident CTAs: exercises the persistent loops)."""
+    """(The name dates from two kernel generations that were compared here; there is one kernel per direction now.)
+    Forward and backward twice on the same inputs and the same dropout stream: same Philox bits, so context,
+    log-sum-exp and all three gradients must agree to bf16 rounding (dQ is reduced over key blocks with fp32
+    reductions whose order is free); a race shows up as a run-to-run difference.  The big case has far more CTAs
+    than the machine holds at once."""
     K = _api()
     torch.manual_seed(2)
     H = heads * 64
@@ -129,19 +103,15 @@ def test_row_kernels_match_round1_kernels(B, S, heads, lens, p_drop):
     seqlens = torch.tensor(lens if lens is not None else [S - (i % 5) * 7 for i in range(B)], device="cuda", dtype=torch.int32)
     dctx = (torch.randn(B, S, H, device="cuda") * 0.5).to(torch.bfloat16)
     kw = dict(p_drop=p_drop, seed=99, stream=6)
-    try:
-        K.set_attention_options(row_kernels=False)
-        ctx0, lse0 = K.attention_fwd(qkv, seqlens, heads, **kw)
-        g0 = K.attention_bwd(qkv, seqlens, ctx0, dctx, lse0, heads, **kw).float()
-        K.set_attention_options(row_kernels=True)
-        for _ in range(2):                                   # twice: races show up as run-to-run differences
-            ctx1, lse1 = K.attention_fwd(qkv, seqlens, heads, **kw)
-            g1 = K.attention_bwd(qkv, seqlens, ctx0, dctx, lse0, heads, **kw).float()
-            torch.cuda.synchronize()
-            valid = (torch.arange(S, device="cuda")[None, :] < seqlens[:, None])            # padded query rows: don't care
-            assert ((ctx1.float() - ctx0.float()).abs() * valid[:, :, None]).max().item() < 2e-2
-            assert ((lse1 - lse0).abs() * valid[:, None, :]).max().item() < 1e-3
-            scale = g0.abs().max().item()
-            assert (g1 - g0).abs().max().item() <= 1.5e-2 * max(scale, 1.0), ((g1 - g0).abs().max().item(), scale)
-    finally:
-        K.set_attention_options(None, None)
+    ctx0, lse0 = K.attention_fwd(qkv, seqlens, heads, **kw)
+    g0 = K.attention_bwd(qkv, seqlens, ctx0, dctx, lse0, heads, **kw).float()
+    for _ in range(2):
+        ctx1, lse1 = K.attention_fwd(qkv, seqlens, heads, **kw)
+        g1 = K.attention_bwd(qkv, seqlens, ctx0, dctx, lse0, heads, **kw).float()
+        torch.cuda.synchronize()
+        valid = (torch.arange(S, device="cuda")[None, :] < seqlens[:, None])            # padded query rows: don't care
+        assert ((ctx1.float() - ctx0.float()).abs() * valid[:, :, None]).max().item() < 2e-2
+        assert ((lse1 - lse0).abs() * valid[:, None, :]).max().item() < 1e-3
+        scale = g0.abs().max().item()
+        assert torch.isfinite(g1).all()
+        assert (g1 - g0).abs().max().item() <= 1.5e-2 * max(scale, 1.0), ((g1 - g0).abs().max().item(), scale)

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs a plain fp32 PyTorch reference of the same op (T3 of SURVEY.md 4.2)."""
+"""wgmma GEMM vs a plain fp32 PyTorch reference of the same op (T3 of SURVEY.md 4.2)."""
 import math
 
 import pytest
@@ -84,8 +84,8 @@ def test_gemm_tn_tail_split(M, N, K):
 @pytest.mark.parametrize("M,N,K,splits", [(4096, 1024, 12288, -2), (1024, 4096, 4096, 1), (512, 512, 1024, -2), (768, 1536, 2048, 3),
                                           (304, 1000, 520, 1)])
 def test_gemm_tn_wide_tiles(M, N, K, splits):
-    """256 x 512 tiles (block_n=1024: two N = 256 MMAs per k-step, all 512 TMEM columns, 4-stage ring of 48 KB) for the
-    fp32 weight-gradient epilogue, alone, with split-K and with the tail split; accumulates into ``out``."""
+    """The widest tiles (128 x 256, 4-stage ring of 48 KB) for the fp32 weight-gradient epilogue, alone, with split-K
+    and with the automatic split (k_splits < 0); accumulates into ``out``."""
     K_ = _ops()
     a, b = _rand(K, M), _rand(K, N)
     out = torch.randn(M, N, device="cuda")
@@ -137,7 +137,7 @@ def test_gemm_dropout_statistics_and_determinism():
 
 
 def test_gemm_pair_many_tiles_and_tails():
-    """More tiles than clusters (persistent loop, TMEM double buffering, ring wrap) and ragged M/N edges."""
+    """More tiles than SMs (several waves of CTAs, ring wrap) and ragged M/N edges."""
     K_ = _ops()
     for (M, N, Kd) in [(12288, 1024, 1024), (1000, 1000, 520), (257, 264, 64), (4096, 30528, 256)]:
         a, b = _rand(M, Kd), _rand(N, Kd)

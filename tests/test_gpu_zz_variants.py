@@ -1,5 +1,5 @@
-"""Model variants next to the flagship config: the no-NSP (RoBERTa-style) model on the fused engine (first run on a
-B200 in round 2: passes) and configurations the kernel program does not implement, which must fall back to the plain
+"""Model variants next to the flagship config: the no-NSP (RoBERTa-style) model on the fused engine
+and configurations the kernel program does not implement, which must fall back to the plain
 PyTorch path instead of raising."""
 import copy
 import os

@@ -104,7 +104,8 @@ def _kfac_gloo_worker(rank, world, port, q):
         for p in base.parameters():
             comm.all_reduce_(p.grad, op="avg")
         k.step()
-    q.put((rank, [p.grad.clone() for p in base.parameters()]))
+    # by value: a tensor in a queue is a file descriptor served by this process, which may exit before the parent reads it
+    q.put((rank, [p.grad.numpy().copy() for p in base.parameters()]))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -122,6 +123,7 @@ def test_kfac_hybrid_groups_over_gloo_four_ranks_match_single_process():
     for p in procs:
         p.start()
     res = sorted([q.get(timeout=180) for _ in range(world)], key=lambda t: t[0])
+    res = [(r, [torch.from_numpy(a) for a in gs]) for r, gs in res]
     for p in procs:
         p.join(timeout=60)
     for r in range(1, world):

@@ -122,7 +122,8 @@ def _gloo_worker(rank, world, port, q):
         ddp.sync_gradients()                      # suppressed inside no_sync
     g_local = arena.flat_grad.clone()
     ddp.sync_gradients()
-    q.put((rank, w0, g_local, arena.flat_grad.clone()))
+    # by value: a tensor in a queue is a file descriptor served by this process, which may exit before the parent reads it
+    q.put((rank, w0.numpy().copy(), g_local.numpy().copy(), arena.flat_grad.numpy().copy()))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -137,7 +138,7 @@ def test_gloo_data_parallel_broadcast_nosync_and_average():
     res = sorted([q.get(timeout=120) for _ in range(world)], key=lambda t: t[0])
     for p in procs:
         p.join(timeout=60)
-    (_, w0a, ga, sa), (_, w0b, gb, sb) = res
+    (_, w0a, ga, sa), (_, w0b, gb, sb) = [(r, *(torch.from_numpy(a) for a in arrs)) for r, *arrs in res]
     assert torch.equal(w0a, w0b)                                   # broadcast at construction
     assert not torch.equal(ga, gb)                                 # no_sync kept gradients local
     assert torch.allclose(sa, (ga + gb) / 2, atol=1e-7) and torch.equal(sa, sb)
@@ -234,7 +235,7 @@ def _hier_worker(rank, world, port, q):
     assert c.inner.rank == rank % 2 and c.inner.world_size == 2
     c.push_master = False
     c.fused_lamb_step(optimizer=None, loss_scale=4.0)
-    q.put((rank, c.inner.result.clone(), c.inner.push_master))
+    q.put((rank, c.inner.result.numpy().copy(), c.inner.push_master))       # by value, as in _gloo_worker
     dist.barrier()
     dist.destroy_process_group()
 
@@ -252,7 +253,7 @@ def test_two_level_fused_backend_composition_gloo():
         p.join(timeout=60)
     for _, out, pm in res:
         assert pm is False
-        assert torch.allclose(out, torch.full((8,), (1 + 2 + 3 + 4) / 4 / 4.0))
+        assert torch.allclose(torch.from_numpy(out), torch.full((8,), (1 + 2 + 3 + 4) / 4 / 4.0))
 
 
 def _ddp_worker(rank, world, port, q):

@@ -1,12 +1,17 @@
-"""Differential tests against the LIVE reference code (CPU): the unmodified reference modules (baseline/_ref or
-/root/reference, with the torch-native shims of baseline/shims standing in for apex / dllogger / ...) run in a
-subprocess on fixed inputs, this repository runs on the same inputs, and the results are compared:
+"""Differential tests against the reference code (CPU): the unmodified reference modules (with the torch-native shims
+of baseline/shims standing in for apex / dllogger / ...) ran on fixed, seeded inputs and what they returned is stored
+under tests/golden/reference_parity/; this repository runs on the same inputs and the results are compared:
 
 * model zoo: the reference's state dict loads strictly into our models; logits agree to float precision
 * tokenizers (BasicTokenizer / WordpieceTokenizer), SQuAD featurisation and n-best post-processing
 * LR schedulers coupled to the optimizer step, BertAdam updates, distributed sampler chunking
 
-Skipped when no copy of the reference is reachable."""
+So are the results of its run_squad.py command line and of its utils/ scripts (tests/golden/reference_tools.pkl.gz)
+and the flag tables of its parsers (reference_cli_flags.json).  To record the golden files again from a copy of the
+reference tree under baseline/_ref:
+
+    python tests/test_reference_parity.py
+"""
 import json
 import os
 import pickle
@@ -18,9 +23,9 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = next((p for p in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference")
+REF = next((p for p in (os.path.join(ROOT, "baseline", "_ref"),)
             if os.path.isfile(os.path.join(p, "src", "modeling.py"))), None)
-pytestmark = pytest.mark.skipif(REF is None, reason="no copy of the reference tree available")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_parity")     # one gzipped pickle per result group
 
 MODEL_CFG = dict(vocab_size=120, hidden_size=32, num_hidden_layers=2, num_attention_heads=4, intermediate_size=64,
                  hidden_act="gelu", hidden_dropout_prob=0.1, attention_probs_dropout_prob=0.1, max_position_embeddings=64,
@@ -454,9 +459,8 @@ pickle.dump(out, open(work + "/ref.pkl", "wb"))
 '''
 
 
-@pytest.fixture(scope="module")
-def ref(tmp_path_factory):
-    work = tmp_path_factory.mktemp("refparity")
+def _write_inputs(work):
+    """The fixed inputs of the comparison (files under ``work`` + the spec the reference script reads)."""
     rng = np.random.default_rng(1)
     ids = rng.integers(5, MODEL_CFG["vocab_size"], size=(3, 24))
     seg = np.zeros_like(ids); seg[:, 12:] = 1
@@ -467,7 +471,7 @@ def ref(tmp_path_factory):
              # (no store_true flag here: the reference's auxiliary parser registers every option as taking a value, so
              #  `--fp16` on its command line is an argparse error -- booleans can only come from the JSON file there)
              ["--config_file", str(work / "train.json"), "--learning_rate", "0.5", "--steps", "12", "--input_dir", "/x"]]
-    ref_utils = next((p for p in (os.path.join(REF, "utils"), "/root/reference/utils") if os.path.isfile(os.path.join(p, "encode_data.py"))), "")
+    ref_utils = os.path.join(REF, "utils") if REF and os.path.isfile(os.path.join(REF, "utils", "encode_data.py")) else ""
     v2 = {"version": "v2.0", "data": [{"title": "t", "paragraphs": [
         {"context": "Hamlet is a play. The play was written by William Shakespeare in 1603.",
          "qas": [{"id": "i1", "question": "Who wrote the river?", "is_impossible": True, "answers": []},
@@ -515,13 +519,55 @@ def ref(tmp_path_factory):
     pickle.dump(spec, open(work / "spec.pkl", "wb"))
     (work / "vocab.txt").write_text("\n".join(VOCAB) + "\n")
     (work / "squad.json").write_text(json.dumps(SQUAD))
+    return spec
+
+
+def _run_reference(work):
+    """Run REF_SCRIPT inside the reference tree on the inputs under ``work`` -> its results, plus the files it wrote
+    under ``work`` (``_files``) and the directory they were recorded in (``_work``)."""
+    before = {os.path.join(d, f) for d, _, fs in os.walk(work) for f in fs}
     (work / "ref_script.py").write_text(REF_SCRIPT)
     env = dict(os.environ, PYTHONPATH=os.path.join(ROOT, "baseline", "shims"), CUDA_VISIBLE_DEVICES="")
     r = subprocess.run([sys.executable, str(work / "ref_script.py"), str(work)], cwd=REF, env=env, capture_output=True,
                        text=True, timeout=600)
     if r.returncode != 0:
-        pytest.skip("the reference code does not run here: " + (r.stderr or r.stdout)[-400:])
+        raise RuntimeError("the reference code does not run here: " + (r.stderr or r.stdout)[-2000:])
     out = pickle.load(open(work / "ref.pkl", "rb"))
+    after = {os.path.join(d, f) for d, _, fs in os.walk(work) for f in fs}
+    out["_files"] = {os.path.relpath(f, work): open(f, "rb").read() for f in sorted(after - before)
+                     if os.path.basename(f) not in ("ref.pkl", "ref_script.py")}
+    out["_work"] = str(work)
+    return out
+
+
+def _rebase(o, old, new):
+    """Every string of a nested result that names the recording directory -> the same path under ``new``."""
+    if isinstance(o, str):
+        return o.replace(old, new)
+    if isinstance(o, bytes):
+        return o.replace(old.encode(), new.encode()) if old.encode() in o else o
+    if isinstance(o, dict):
+        return {k: _rebase(v, old, new) for k, v in o.items()}
+    if isinstance(o, list):
+        return [_rebase(v, old, new) for v in o]
+    if isinstance(o, tuple):
+        return tuple(_rebase(v, old, new) for v in o)
+    return o
+
+
+@pytest.fixture(scope="module")
+def ref(tmp_path_factory):
+    import gzip
+    work = tmp_path_factory.mktemp("refparity")
+    spec = _write_inputs(work)
+    out = {}
+    for f in sorted(os.listdir(GOLDEN)):
+        with gzip.open(os.path.join(GOLDEN, f), "rb") as g:
+            out[f[:-len(".pkl.gz")]] = pickle.load(g)
+    out = _rebase(out, out.pop("_work"), str(work))
+    for rel, data in out.pop("_files").items():
+        os.makedirs(os.path.dirname(work / rel), exist_ok=True)
+        (work / rel).write_bytes(data)
     out["work"], out["spec"] = str(work), spec
     return out
 
@@ -802,32 +848,129 @@ def test_training_steps_agree(ref):
     assert worst < 5e-5, worst
 
 
-def test_run_squad_predict_cli_end_to_end(ref, tmp_path):
-    """Both run_squad.py command lines (the reference's and this repo's), same checkpoint, prediction only on the CPU:
-    identical predictions.json and n-best lists (CLI -> checkpoint load -> features -> forward -> post-processing)."""
-    from bert_pytorch_b200 import BertConfig, finetune_squad, models as M
-    work = ref["work"]
+TOOLS_GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_tools.pkl.gz")   # what _record_tools() returned
+
+
+def _tools_golden():
+    import gzip
+    with gzip.open(TOOLS_GOLDEN, "rb") as f:
+        return pickle.load(f)
+
+
+def _load_ref_util(name):
+    """The reference's utils/<name>.py as a module (recording only; the h5py stand-in serves its imports)."""
+    import importlib.util
+    sys.path.insert(0, os.path.join(ROOT, "baseline", "shims"))
+    try:
+        spec = importlib.util.spec_from_file_location("ref_" + name, os.path.join(REF, "utils", name + ".py"))
+        mod = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(mod)
+    finally:
+        sys.path.pop(0)
+    return mod
+
+
+def _squad_cli_args(work, tmp_path, state_dict):
+    """Model JSON + checkpoint + the prediction-only command line."""
     cfg = dict(MODEL_CFG, hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0,
                vocab_file=os.path.join(work, "vocab.txt"), tokenizer="wordpiece", lowercase=True)
     model_json = str(tmp_path / "model.json")
     json.dump(cfg, open(model_json, "w"))
-    torch.manual_seed(5)
     ckpt = str(tmp_path / "ckpt_10.pt")
-    torch.save({"model": M.BertForPreTraining(BertConfig.from_dict(cfg)).state_dict()}, ckpt)
-    common = ["--no_cuda", "--bert_model", "bert-large-uncased", "--init_checkpoint", ckpt, "--config_file", model_json,
-              "--vocab_file", cfg["vocab_file"], "--do_predict", "--predict_file", os.path.join(work, "squad.json"),
-              "--predict_batch_size", "4", "--max_seq_length", "48", "--doc_stride", "16", "--max_query_length", "12",
-              "--do_lower_case", "--seed", "42"]
+    torch.save({"model": {k: torch.from_numpy(np.array(v)) for k, v in state_dict.items()}}, ckpt)
+    return ["--no_cuda", "--bert_model", "bert-large-uncased", "--init_checkpoint", ckpt, "--config_file", model_json,
+            "--vocab_file", cfg["vocab_file"], "--do_predict", "--predict_file", os.path.join(work, "squad.json"),
+            "--predict_batch_size", "4", "--max_seq_length", "48", "--doc_stride", "16", "--max_query_length", "12",
+            "--do_lower_case", "--seed", "42"]
+
+
+SHARD_TEXT = "".join(f"Article {i} sentence one.\nArticle {i} sentence two is a little longer than one.\n\n" for i in range(40))
+SAMPLE_TEXT = "".join("".join(f"Article {i} sentence {j}.\n" for j in range(1 + i % 4)) + "\n" for i in range(60))
+SIZE_VALUES = (5, "123", "2K", "1.5M", "3b")
+WRITER_RAW = [([5, 6, 7], [8, 9], True), ([10], [11, 12, 13, 14], False), ([20, 21, 22, 23, 24], [25], False)]
+
+
+def _packer_docs():
+    import random
+    gen = random.Random(5)
+    return [[[gen.randrange(10, 500) for _ in range(gen.randint(1, 30))] for _ in range(gen.randint(1, 12))] for _ in range(9)]
+
+
+def _read_dir(d):
+    return {f: open(os.path.join(d, f)).read() for f in sorted(os.listdir(d))}
+
+
+def _record_tools(work, tmp_path):
+    """Run the reference's run_squad.py command line and its utils/ scripts on the fixed inputs of the tests below."""
+    import random
+    from bert_pytorch_b200 import BertConfig, models as M
+    out = {}
+    torch.manual_seed(5)                                  # the checkpoint both command lines predict from
+    out["squad_ckpt"] = {k: v.numpy().copy() for k, v in M.BertForPreTraining(BertConfig.from_dict(
+        dict(MODEL_CFG, hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0))).state_dict().items()}
+    common = _squad_cli_args(str(work), tmp_path, out["squad_ckpt"])
     env = dict(os.environ, PYTHONPATH=os.path.join(ROOT, "baseline", "shims"), CUDA_VISIBLE_DEVICES="")
     r = subprocess.run([sys.executable, "run_squad.py", *common, "--output_dir", str(tmp_path / "ref_out")], cwd=REF, env=env,
                        capture_output=True, text=True, timeout=600)
-    if r.returncode != 0:
-        pytest.skip("the reference runner does not run here: " + (r.stderr or r.stdout)[-300:])
+    assert r.returncode == 0, (r.stderr or r.stdout)[-2000:]
+    out["squad_predictions"] = json.load(open(tmp_path / "ref_out" / "predictions.json"))
+    out["squad_nbest"] = {k: [{"text": x["text"], "probability": x["probability"]} for x in v]
+                          for k, v in json.load(open(tmp_path / "ref_out" / "nbest_predictions.json")).items()}
+    RSH = _load_ref_util("shard")
+    src = tmp_path / "shard_in.txt"
+    src.write_text(SHARD_TEXT)
+    out["shard"] = {}
+    for limit in (None, 3):
+        d = tmp_path / f"shard_ref_{limit}"
+        d.mkdir()
+        RSH.shard(str(src), str(d / "shard_{index}.txt"), 700, limit)
+        out["shard"][limit] = _read_dir(d)
+    out["shard_sizes"] = {repr(v): RSH.parse_value_as_int(v) for v in SIZE_VALUES}
+    src = tmp_path / "sample_in.txt"
+    src.write_text(SAMPLE_TEXT)
+    code = ("import random, runpy, sys; random.seed(11); sys.argv = ['sample_and_shard.py', '-i', sys.argv[1], '-o', sys.argv[2], "
+            "'-b', '400', '-n', '50']; runpy.run_path(%r, run_name='__main__')" % os.path.join(REF, "utils", "sample_and_shard.py"))
+    r = subprocess.run([sys.executable, "-c", code, str(src), str(tmp_path / "sample_ref")], capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, r.stderr[-500:]
+    out["sample_and_shard"] = _read_dir(tmp_path / "sample_ref")
+    E = _load_ref_util("encode_data")
+    docs_ref = [[[f"t{t}" for t in sent] for sent in d] for d in _packer_docs()]
+    out["packing"] = {}
+    for nsp in (0.5, 0.0):
+        for seed in range(6):
+            random.seed(seed)
+            want = []
+            for i in range(len(docs_ref)):
+                want.extend(E.create_samples_from_document(i, docs_ref, 48, nsp, 0.3))
+            random.shuffle(want)
+            out["packing"][(nsp, seed)] = [(w.seq_tokens, w.next_seq_tokens, w.is_random_next, w.special_token_positions,
+                                            len(w.sequence)) for w in want]
+    from bert_pytorch_b200.data import hdf5
+
+    class Tok:                                            # "t17" -> 17, specials like a real vocabulary
+        def token_to_id(self, t):
+            return {"[CLS]": 101, "[SEP]": 102}.get(t) or int(t[1:])
+    out["writer"] = {}
+    for nsp in (True, False):
+        samples = [E.TrainingSample([f"t{x}" for x in a], [f"t{x}" for x in b] if nsp else None, r and nsp) for a, b, r in WRITER_RAW]
+        fa = str(tmp_path / f"writer_ref_{nsp}.hdf5")
+        E.write_samples_to_hdf5(fa, list(samples), Tok(), 16)
+        with hdf5.File(fa, "r") as A:
+            out["writer"][nsp] = {k: A[k][:] for k in A.keys()}
+    return out
+
+
+def test_run_squad_predict_cli_end_to_end(ref, tmp_path):
+    """Both run_squad.py command lines (the reference's, recorded, and this repo's), same checkpoint, prediction only on
+    the CPU: identical predictions.json and n-best lists (CLI -> checkpoint load -> features -> forward -> post-processing)."""
+    from bert_pytorch_b200 import finetune_squad
+    gold = _tools_golden()
+    common = _squad_cli_args(ref["work"], tmp_path, gold["squad_ckpt"])
     finetune_squad.main([*common, "--output_dir", str(tmp_path / "my_out")])
-    a = json.load(open(tmp_path / "ref_out" / "predictions.json"))
+    a = gold["squad_predictions"]
     b = json.load(open(tmp_path / "my_out" / "predictions.json"))
     assert a == b and {"q1", "q2", "q3"} <= set(a) and len(a) >= 15
-    na = json.load(open(tmp_path / "ref_out" / "nbest_predictions.json"))
+    na = gold["squad_nbest"]
     nb = json.load(open(tmp_path / "my_out" / "nbest_predictions.json"))
     for k in na:
         # logits come out of two implementations of the forward pass (agreement ~1e-6): candidates whose scores are
@@ -841,51 +984,34 @@ def test_run_squad_predict_cli_end_to_end(ref, tmp_path):
 def test_text_sharder_agrees(tmp_path):
     """utils/shard.py: same shard files for the same input (split at the first article boundary past the byte budget,
     1-based names, optional shard limit) and the same size parser."""
-    import importlib.util
-    ref_utils = next((p for p in (os.path.join(REF, "utils"), "/root/reference/utils") if os.path.isfile(os.path.join(p, "shard.py"))), None)
-    if ref_utils is None:
-        pytest.skip("the reference's utils/ directory is not available")
-    spec = importlib.util.spec_from_file_location("ref_shard", os.path.join(ref_utils, "shard.py"))
-    RSH = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(RSH)
     from bert_pytorch_b200.data import corpus
-    text = "".join(f"Article {i} sentence one.\nArticle {i} sentence two is a little longer than one.\n\n" for i in range(40))
+    gold = _tools_golden()
     src = tmp_path / "in.txt"
-    src.write_text(text)
+    src.write_text(SHARD_TEXT)
     for limit in (None, 3):
-        a, b = tmp_path / f"ref_{limit}", tmp_path / f"mine_{limit}"
-        a.mkdir(); b.mkdir()
-        RSH.shard(str(src), str(a / "shard_{index}.txt"), 700, limit)
+        b = tmp_path / f"mine_{limit}"
+        b.mkdir()
         corpus.shard_text(str(src), str(b / "shard_{index}.txt"), 700, limit)
-        fa, fb = sorted(os.listdir(a)), sorted(os.listdir(b))
-        assert fa == fb and len(fa) >= 3, (fa, fb)
-        for f in fa:
-            assert (a / f).read_text() == (b / f).read_text(), (limit, f)
-    for v in (5, "123", "2K", "1.5M", "3b"):
-        assert corpus.parse_value_as_int(v) == RSH.parse_value_as_int(v), v
+        want, got = gold["shard"][limit], _read_dir(b)
+        assert sorted(want) == sorted(got) and len(want) >= 3, (sorted(want), sorted(got))
+        for f in want:
+            assert want[f] == got[f], (limit, f)
+    for v in SIZE_VALUES:
+        assert corpus.parse_value_as_int(v) == gold["shard_sizes"][repr(v)], v
 
 
 def test_sample_and_shard_agrees(tmp_path):
     """utils/sample_and_shard.py under the same `random` seed: the same articles in the same shard files."""
     import random
-    ref_utils = next((p for p in (os.path.join(REF, "utils"), "/root/reference/utils")
-                      if os.path.isfile(os.path.join(p, "sample_and_shard.py"))), None)
-    if ref_utils is None:
-        pytest.skip("the reference's utils/ directory is not available")
     from bert_pytorch_b200.data import corpus
     src = tmp_path / "in.txt"
-    src.write_text("".join("".join(f"Article {i} sentence {j}.\n" for j in range(1 + i % 4)) + "\n" for i in range(60)))
-    a, b = tmp_path / "ref", tmp_path / "mine"
-    code = ("import random, runpy, sys; random.seed(11); sys.argv = ['sample_and_shard.py', '-i', sys.argv[1], '-o', sys.argv[2], "
-            "'-b', '400', '-n', '50']; runpy.run_path(sys.argv[0] if False else %r, run_name='__main__')"
-            % os.path.join(ref_utils, "sample_and_shard.py"))
-    r = subprocess.run([sys.executable, "-c", code, str(src), str(a)], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr[-500:]
+    src.write_text(SAMPLE_TEXT)
+    b = tmp_path / "mine"
     corpus.sample_and_shard([str(src)], str(b / "shard_{index}.txt"), 400, 50, random.Random(11))
-    fa, fb = sorted(os.listdir(a)), sorted(os.listdir(b))
-    assert fa == fb and len(fa) >= 2, (fa, fb)
-    for f in fa:
-        assert (a / f).read_text() == (b / f).read_text(), f
+    want, got = _tools_golden()["sample_and_shard"], _read_dir(b)
+    assert sorted(want) == sorted(got) and len(want) >= 2, (sorted(want), sorted(got))
+    for f in want:
+        assert want[f] == got[f], f
 
 
 @pytest.mark.parametrize("next_seq_prob", [0.5, 0.0])
@@ -893,37 +1019,20 @@ def test_sample_packing_agrees_draw_for_draw(next_seq_prob):
     """utils/encode_data.py:create_samples_from_document under the same `random` seed: the packer makes the same random
     decisions in the same order (target lengths, A/B cut, random-next documents, re-use of displaced sentences, final
     shuffle), so the samples are identical."""
-    import importlib.util
     import random
-    ref_utils = next((p for p in (os.path.join(REF, "utils"), "/root/reference/utils")
-                      if os.path.isfile(os.path.join(p, "encode_data.py"))), None)
-    if ref_utils is None:
-        pytest.skip("the reference's utils/ directory is not available")
-    sys.path.insert(0, os.path.join(ROOT, "baseline", "shims"))          # h5py stand-in for the import
-    try:
-        spec = importlib.util.spec_from_file_location("ref_encode_data2", os.path.join(ref_utils, "encode_data.py"))
-        E = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(E)
-    finally:
-        sys.path.pop(0)
     from bert_pytorch_b200.data.encode import SamplePacker
-    gen = random.Random(5)
-    docs = [[[gen.randrange(10, 500) for _ in range(gen.randint(1, 30))] for _ in range(gen.randint(1, 12))] for _ in range(9)]
-    docs_ref = [[[f"t{t}" for t in sent] for sent in d] for d in docs]
+    gold = _tools_golden()["packing"]
+    docs = _packer_docs()
     for seed in range(6):
-        random.seed(seed)
-        want = []
-        for i in range(len(docs_ref)):
-            want.extend(E.create_samples_from_document(i, docs_ref, 48, next_seq_prob, 0.3))
-        random.shuffle(want)
+        want = gold[(next_seq_prob, seed)]
         got = SamplePacker(48, next_seq_prob, 0.3, random.Random(seed)).pack_file(docs)
         assert len(got) == len(want), seed
-        for g, w in zip(got, want):
-            assert [f"t{t}" for t in g.seq_ids] == w.seq_tokens, seed
-            assert (None if g.next_seq_ids is None else [f"t{t}" for t in g.next_seq_ids]) == w.next_seq_tokens, seed
-            assert g.is_random_next == w.is_random_next
+        for g, (w_seq, w_next, w_random, w_special, w_len) in zip(got, want):
+            assert [f"t{t}" for t in g.seq_ids] == w_seq, seed
+            assert (None if g.next_seq_ids is None else [f"t{t}" for t in g.next_seq_ids]) == w_next, seed
+            assert g.is_random_next == w_random
             ids, special = g.layout(1, 2)
-            assert special == w.special_token_positions and len(ids) == len(w.sequence) <= 48
+            assert special == w_special and len(ids) == w_len <= 48
 
 
 def test_dynamic_masking_statistics_agree(ref):
@@ -1000,34 +1109,17 @@ def test_shard_writer_agrees(tmp_path):
     """utils/encode_data.py:write_samples_to_hdf5 (the reference, writing through the h5py stand-in = this repo's HDF5
     writer) and data/encode.py write the same three datasets for the same samples (the reference pops from the end of the
     list, so its rows come out reversed)."""
-    import importlib.util
-    ref_utils = next((p for p in (os.path.join(REF, "utils"), "/root/reference/utils")
-                      if os.path.isfile(os.path.join(p, "encode_data.py"))), None)
-    if ref_utils is None:
-        pytest.skip("the reference's utils/ directory is not available")
-    sys.path.insert(0, os.path.join(ROOT, "baseline", "shims"))
-    try:
-        spec = importlib.util.spec_from_file_location("ref_encode_data3", os.path.join(ref_utils, "encode_data.py"))
-        E = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(E)
-    finally:
-        sys.path.pop(0)
     from bert_pytorch_b200.data import encode, hdf5
-
-    class Tok:                                            # "t17" -> 17, specials like a real vocabulary
-        def token_to_id(self, t):
-            return {"[CLS]": 101, "[SEP]": 102}.get(t) or int(t[1:])
-    raw = [([5, 6, 7], [8, 9], True), ([10], [11, 12, 13, 14], False), ([20, 21, 22, 23, 24], [25], False)]
+    gold = _tools_golden()["writer"]
     for nsp in (True, False):
-        ref_samples = [E.TrainingSample([f"t{x}" for x in a], [f"t{x}" for x in b] if nsp else None, r and nsp) for a, b, r in raw]
-        mine = [encode.TrainingSample(list(a), list(b) if nsp else None, r and nsp) for a, b, r in raw]
-        fa, fb = str(tmp_path / f"ref_{nsp}.hdf5"), str(tmp_path / f"mine_{nsp}.hdf5")
-        E.write_samples_to_hdf5(fa, list(ref_samples), Tok(), 16)
+        mine = [encode.TrainingSample(list(a), list(b) if nsp else None, r and nsp) for a, b, r in WRITER_RAW]
+        fb = str(tmp_path / f"mine_{nsp}.hdf5")
         encode.write_samples_to_hdf5(fb, mine, 16, 101, 102)
-        with hdf5.File(fa, "r") as A, hdf5.File(fb, "r") as B:
+        A = gold[nsp]
+        with hdf5.File(fb, "r") as B:
             assert sorted(A.keys()) == sorted(B.keys()) == ["input_ids", "next_sentence_labels", "special_token_positions"]
             for k in A.keys():
-                a, b = A[k][:], B[k][:]
+                a, b = A[k], B[k][:]
                 assert a.dtype == b.dtype and a.shape == b.shape, (k, a.dtype, b.dtype, a.shape, b.shape)
                 assert np.array_equal(a[::-1], b), k
 
@@ -1160,41 +1252,6 @@ def test_activation_table_and_linear_activation_agree(ref):
         assert np.allclose(m(x).detach().numpy(), want, atol=1e-6, rtol=1e-5), act
 
 
-def test_run_squad_flags_and_defaults_agree():
-    """run_squad.py builds its parser inside main(); its add_argument calls are read from the source (AST) and compared
-    with this repo's parser: every flag exists with the same default, type and store_true behaviour."""
-    import ast
-    from bert_pytorch_b200 import finetune_squad
-    tree = ast.parse(open(os.path.join(REF, "run_squad.py")).read())
-    ref = {}
-    for node in ast.walk(tree):
-        if isinstance(node, ast.Call) and isinstance(node.func, ast.Attribute) and node.func.attr == "add_argument":
-            names = [a.value for a in node.args if isinstance(a, ast.Constant) and isinstance(a.value, str)]
-            if not names:
-                continue
-            kw = {}
-            for k in node.keywords:
-                if k.arg in ("default", "action"):
-                    try:
-                        kw[k.arg] = ast.literal_eval(k.value)
-                    except ValueError:
-                        kw[k.arg] = None                         # computed default (LOCAL_RANK from the environment)
-                elif k.arg == "type" and isinstance(k.value, ast.Name):
-                    kw["type"] = k.value.id
-            ref[names[-1].lstrip("-").replace("-", "_")] = kw
-    assert len(ref) >= 40
-    mine = {a.dest: a for a in finetune_squad.build_parser()._actions}
-    assert not [k for k in ref if k not in mine]
-    for k, kw in ref.items():
-        a = mine[k]
-        if kw.get("default", None) is not None:
-            assert a.default == kw["default"], (k, a.default, kw["default"])
-        if kw.get("action") == "store_true":
-            assert a.nargs == 0 and a.const is True and a.default is False, k
-        if kw.get("type") in ("int", "float", "str") and a.type is not None:
-            assert a.type.__name__ == kw["type"], k
-
-
 def _argparse_table(path):
     """flag -> (default, type name, action) of every add_argument call in a source file (AST, nothing is executed)."""
     import ast
@@ -1217,12 +1274,31 @@ def _argparse_table(path):
     return table
 
 
-@pytest.mark.parametrize("script", ["encode_data.py", "format.py", "download.py", "build_vocab.py", "shard.py", "sample_and_shard.py"])
+FLAGS_GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_cli_flags.json")   # _argparse_table of the reference's scripts
+DATA_TOOLS = ["encode_data.py", "format.py", "download.py", "build_vocab.py", "shard.py", "sample_and_shard.py"]
+
+
+def test_run_squad_flags_and_defaults_agree():
+    """run_squad.py builds its parser inside main(); its add_argument calls were read from the source (AST) and are
+    compared with this repo's parser: every flag exists with the same default, type and store_true behaviour."""
+    from bert_pytorch_b200 import finetune_squad
+    ref = json.load(open(FLAGS_GOLDEN))["run_squad.py"]
+    assert len(ref) >= 40
+    mine = {a.dest: a for a in finetune_squad.build_parser()._actions}
+    assert not [k for k in ref if k not in mine]
+    for k, kw in ref.items():
+        a = mine[k]
+        if kw["default"] not in (None, "<computed>"):            # computed: LOCAL_RANK from the environment
+            assert a.default == kw["default"], (k, a.default, kw["default"])
+        if kw["action"] == "store_true":
+            assert a.nargs == 0 and a.const is True and a.default is False, k
+        if kw["type"] in ("int", "float", "str") and a.type is not None:
+            assert a.type.__name__ == kw["type"], k
+
+
+@pytest.mark.parametrize("script", DATA_TOOLS)
 def test_data_tool_flags_and_defaults_agree(script):
-    ref_utils = next((p for p in (os.path.join(REF, "utils"), "/root/reference/utils") if os.path.isfile(os.path.join(p, script))), None)
-    if ref_utils is None:
-        pytest.skip("the reference's utils/ directory is not available")
-    ref, mine = _argparse_table(os.path.join(ref_utils, script)), _argparse_table(os.path.join(ROOT, "utils", script))
+    ref, mine = json.load(open(FLAGS_GOLDEN))["utils/" + script], _argparse_table(os.path.join(ROOT, "utils", script))
     assert ref, script
     for flag, kw in ref.items():
         assert flag in mine, (script, flag)
@@ -1233,3 +1309,30 @@ def test_data_tool_flags_and_defaults_agree(script):
             assert m["action"] == "store_true", (script, flag)
         if kw["type"] in ("int", "float", "str") and m["type"] is not None:
             assert m["type"] == kw["type"], (script, flag)
+
+
+if __name__ == "__main__":                     # record tests/golden/reference_parity/ from baseline/_ref
+    import gzip
+    import pathlib
+    import shutil
+    import tempfile
+    assert REF is not None, "needs a copy of the reference tree under baseline/_ref"
+    with tempfile.TemporaryDirectory() as tmp:
+        w = pathlib.Path(tmp)
+        _write_inputs(w)
+        res = _run_reference(w)
+        (w / "tools").mkdir()
+        tools = _rebase(_record_tools(w, w / "tools"), str(w), "<work>")
+    with gzip.GzipFile(TOOLS_GOLDEN, "wb", mtime=0) as f:
+        pickle.dump(tools, f, protocol=4)
+    shutil.rmtree(GOLDEN, ignore_errors=True)
+    os.makedirs(GOLDEN)
+    for key, val in res.items():
+        with gzip.GzipFile(os.path.join(GOLDEN, key + ".pkl.gz"), "wb", mtime=0) as f:
+            pickle.dump(val, f, protocol=4)
+    print(GOLDEN, sum(os.path.getsize(os.path.join(GOLDEN, f)) for f in os.listdir(GOLDEN)), "bytes")
+    flags = {"run_squad.py": _argparse_table(os.path.join(REF, "run_squad.py"))}
+    for tool in DATA_TOOLS:
+        flags["utils/" + tool] = _argparse_table(os.path.join(REF, "utils", tool))
+    with open(FLAGS_GOLDEN, "w") as f:
+        json.dump(flags, f, indent=1, sort_keys=True)

@@ -2,10 +2,10 @@
 schedule through three execution paths -- VERDICT r1 #7 / #8:
 
     oracle-fp32   plain PyTorch autograd, fp32 everywhere (bert.use_fused = False)
-    fused-bf16    the sm_100a kernel program (bf16 operands, fp32 accumulate / master weights)
+    fused-bf16    the sm_90a kernel program (bf16 operands, fp32 accumulate / master weights)
     fused-fp8     same engine with per-tensor delayed-scaling fp8 GEMM operands (e4m3 fwd / e5m2 grads)
 
-    python tools/convergence.py [--steps 300] [--hidden 1024 --layers 4] > profiles/convergence_r2.jsonl
+    python tools/convergence.py [--steps 300] [--hidden 1024 --layers 4] > convergence.jsonl
 
 One JSON line per arm with the per-step MLM+NSP loss (dropout off so the three arms see the same function), then a
 summary line with the final-loss ratios (mean of the last 10 % of the steps)."""

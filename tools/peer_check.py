@@ -219,11 +219,11 @@ def main():
         a_r.flat_grad.normal_()
         out["nccl_allreduce_plus_lamb_ms"] = round(timeit(run_ref), 3)
         n = a_r.numel
-        link = 770e9   # measured peer bandwidth per direction (B200_PROFILING.md)
+        link = 450e9   # NVLink 4 data-sheet bandwidth per direction (H100 SXM), not a measured rate
         rs_bytes = 4.0 * n * (world - 1) / world          # gradient shards pulled from the peers
         ag_bytes = 6.0 * n * (world - 1) / world          # fp32 + bf16 pushed to the peers
         out["roofline_ms_nvlink"] = round(max(rs_bytes, ag_bytes) / link * 1e3, 3)
-        hbm = 6.5e12                                      # measured copy bandwidth (MEASURED_PEAKS.json)
+        hbm = 3.35e12                                     # HBM3 data-sheet bandwidth (H100 SXM), not a measured rate
         lamb_bytes = (28.0 + 18.0) * n / world            # phase B (g,p,m,v in; m,v,u out) + phase C local traffic + zeroing share
         # the three phases depend on each other (global norm, trust ratios): their times add up
         out["roofline_ms_serial"] = round((rs_bytes / link + lamb_bytes / hbm + 4.0 * n / hbm + ag_bytes / link) * 1e3, 3)
