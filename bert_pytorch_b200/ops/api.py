@@ -23,9 +23,10 @@ NUM_SMS = 132           # H100 SXM; only the tile heuristics below use it (the k
 KERNEL_LAUNCHES = 0     # every wrapper bumps this: bench.py reports it as ``gpu_launches``
 
 
-def pick_block_n(M: int, N: int) -> int:
-    """The tile width :func:`gemm` chooses for an [M, N] output (128 x 256 or 128 x 128 tiles)."""
-    return _pick_block_n(M, N)
+def pick_block_n(M: int, N: int, epi: int = EPI_NONE) -> int:
+    """The tile width :func:`gemm` chooses for an [M, N] output with epilogue ``epi`` (128 x 256 or 128 x 128
+    tiles)."""
+    return _pick_block_n(M, N, epi)
 
 
 def _count(n: int = 1) -> None:
@@ -33,10 +34,16 @@ def _count(n: int = 1) -> None:
     KERNEL_LAUNCHES += n
 
 
-def _pick_block_n(M: int, N: int) -> int:
-    """256 (128 x 256 tiles: half the A-operand traffic per FLOP) unless the narrow tiles waste clearly fewer SM
-    slots in the last wave; 128 for N <= 128."""
-    if N <= 128:
+# epilogues that read or write a second [M, N] tensor (residual, GELU input or output, keep bits): on 128 x 128 tiles
+# the kernel runs them ping-pong, under the other warpgroup's MMAs, which measured 5-15 % faster on H100 at the
+# BERT-large shapes than the 128 x 256 tile whose two warpgroups run the epilogue together (tools/gemm_bench.py --epi)
+_HEAVY_EPI = (EPI_BIAS_GELU, EPI_BIAS_DROP_RES, EPI_ADD, EPI_DGELU, EPI_BIAS_GELU_DG, EPI_MUL)
+
+
+def _pick_block_n(M: int, N: int, epi: int = EPI_NONE) -> int:
+    """128 for N <= 128 and for the heavy epilogues; otherwise 256 (128 x 256 tiles: half the A-operand traffic per
+    FLOP) unless the narrow tiles waste clearly fewer SM slots in the last wave."""
+    if N <= 128 or epi in _HEAVY_EPI:
         return 128
     m_blocks = (M + 127) // 128
     t256 = m_blocks * ((N + 255) // 256)
@@ -72,7 +79,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, layout: int = NT, epi: int = EPI_N
         dt = torch.float32 if epi in (EPI_ACCUM_F32, EPI_F32) else torch.bfloat16
         out = torch.empty(M, N, dtype=dt, device=a.device)
     if block_n is None:
-        block_n = _pick_block_n(M, N)
+        block_n = _pick_block_n(M, N, epi)
     extension().gemm(a, b, out, layout, epi, bias, res, aux_out, k_splits, block_n, alpha, p_drop, seed, stream,
                      scale_a, scale_b, a_e5m2, b_e5m2, push, colsum, mask_out, mask_in)
     _count()
@@ -124,10 +131,12 @@ class Fp8Meta:
 
 
 def wgrad_splits(n_out: int, k_out: int, reduce_len: int, block_n: int = 256) -> int:
-    """Split-K factor for dW[n_out, k_out] so the grid covers the machine."""
+    """Split-K factor for dW[n_out, k_out]: as many K ranges as keep the work units (tiles x splits) within one unit
+    per SM of the persistent grid.  More splits only add fp32 reduction traffic once every SM has a unit, and a
+    fraction of a second unit per SM leaves the others idle for a whole unit."""
     tiles = ((n_out + 127) // 128) * ((k_out + block_n - 1) // block_n)
     kb = max(1, (reduce_len + 63) // 64)
-    want = max(1, round(2 * NUM_SMS / max(tiles, 1)))
+    want = max(1, NUM_SMS // max(tiles, 1))
     return max(1, min(want, kb // 4 if kb >= 8 else 1, 32))
 
 

@@ -2,11 +2,16 @@
 //
 //   D[M,N] = epilogue( A[M,K] * B[N,K]^T )        bf16 (or fp8) operands, fp32 accumulation in registers
 //
-// One CTA per 128 x BLOCK_N output tile (and K split).  Warpgroup 0 is the producer: one thread moves operand tiles
-// global -> shared memory with cp.async.bulk.tensor (TMA, 128B swizzle) through a STAGES-deep mbarrier ring.
-// Warpgroups 1 and 2 each own 64 rows of the tile: they issue wgmma.mma_async straight from the ring, keep one
-// group in flight, hand a slot back as soon as the group that read it has retired, and run the epilogue from their
-// accumulator registers.
+// Persistent: a work unit is one 128 x BLOCK_N output tile and K range, and min(units, SMs) CTAs each walk the units
+// blockIdx.x, blockIdx.x + gridDim.x, ...  Warpgroup 0 is the producer: one thread moves operand tiles global ->
+// shared memory with cp.async.bulk.tensor (TMA, 128B swizzle) through a STAGES-deep mbarrier ring, running straight
+// across unit boundaries, so the next unit's operands arrive while the consumers are still in an epilogue.
+// Warpgroups 1 and 2 issue wgmma.mma_async straight from the ring, keep one group in flight, hand a slot back as soon
+// as the group that read it has retired, and run the epilogue from their accumulator registers.  Two schedules:
+//   BLOCK_N 256, cooperative: both warpgroups work on every unit, 64 rows each (half the A traffic per FLOP of
+//                128 x 128; the tensor cores idle while both run the epilogue).
+//   BLOCK_N 128, ping-pong:   the warpgroups take alternate units, each the whole 128 x 128 tile, and a pair of named
+//                barriers orders their main loops, so one warpgroup's epilogue runs under the other's MMAs.
 //
 // Both bf16 operands can be K-major (reduction dim contiguous) or MN-major, selected per instantiation, so the same
 // kernel serves the three GEMMs of a linear layer without any transpose copy:
@@ -49,6 +54,7 @@ struct Cfg {
 struct GemmArgs {
   int M, N, K;
   int m_blocks, n_blocks, k_blocks, k_splits, k_per_split;
+  int units;                 // m_blocks * n_blocks * k_splits
   int epi;
   void* out;
   int ldo;
@@ -197,26 +203,50 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
   }
 }
 
-// main loop of one consumer warpgroup: acc (+)= A[64 rows] * B over k-blocks [kb0, kb1)
-template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int AE5, int BE5>
-__device__ __forceinline__ void consumer_mainloop(float (&acc)[BLOCK_N / 2], uint8_t* smem, uint64_t* full_bar,
-                                                  uint64_t* empty_bar, int wg, int nkb) {
+// Work unit u of a launch: output tile (mb, nb) and k-blocks [kb0, kb0 + nkb) -- split-major, then m-block, then
+// n-block, so the units that run at the same time share their A rows in L2.
+struct Unit {
+  int mb, nb, ks, kb0, nkb;
+};
+__device__ __forceinline__ Unit unit_of(const GemmArgs& p, int u) {
+  Unit w;
+  w.nb = u % p.n_blocks;
+  w.mb = (u / p.n_blocks) % p.m_blocks;
+  w.ks = u / (p.n_blocks * p.m_blocks);
+  w.kb0 = w.ks * p.k_per_split;
+  w.nkb = min(p.k_blocks, w.kb0 + p.k_per_split) - w.kb0;   // >= 1: the launcher leaves no empty split
+  return w;
+}
+
+// Main loop of one consumer warpgroup over one unit: acc[r] (+)= A[64 rows, chunk a_chunk + r] * B over the unit's
+// nkb k-blocks, which sit at ring positions it, it + 1, ...  `arrive_bar` >= 0: once every MMA is issued, let the
+// other warpgroup start its main loop (ping-pong order).
+template <bool A_MN, bool B_MN, int BLOCK_N, int R, bool FP8, int AE5, int BE5>
+__device__ __forceinline__ void consumer_mainloop(float (&acc)[R][BLOCK_N / 2], uint8_t* smem, uint64_t* full_bar,
+                                                  uint64_t* empty_bar, int a_chunk, uint32_t it, int nkb,
+                                                  int arrive_bar) {
   using C = Cfg<BLOCK_N>;
   const int lane = threadIdx.x & 31;
-  int s = 0, prev = -1;
-  uint32_t ph = 0;
+  int s = it % C::STAGES, prev = -1;
+  uint32_t ph = (it / C::STAGES) & 1;
+#pragma unroll
+  for (int r = 0; r < R; ++r) wgmma_fence_regs(acc[r]);
   for (int i = 0; i < nkb; ++i) {
     mbar_wait_mma(&full_bar[s], ph);
-    const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES) + wg * 8192;   // this warpgroup's 64 rows (or 64-wide MN chunk)
+    const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES) + a_chunk * 8192;   // 64 rows (or a 64-wide MN chunk) of A
     const uint32_t sb = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       // advance inside the tile: K-major +32 B per MMA (16 bf16 / 32 fp8), MN-major +16 k-rows * 128 B
-      const uint64_t da = A_MN ? wgmma_desc_sw128(sa + kk * 2048, 8192, 1024) : wgmma_desc_sw128(sa + kk * 32, 16, 1024);
       const uint64_t db = B_MN ? wgmma_desc_sw128(sb + kk * 2048, 8192, 1024) : wgmma_desc_sw128(sb + kk * 32, 16, 1024);
-      if constexpr (FP8) WgmmaFp8SS<BLOCK_N, AE5, BE5>::mma(acc, da, db, (i > 0 || kk > 0) ? 1 : 0);
-      else WgmmaBf16SS<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, da, db, (i > 0 || kk > 0) ? 1 : 0);
+#pragma unroll
+      for (int r = 0; r < R; ++r) {
+        const uint32_t sr = sa + r * 8192;
+        const uint64_t da = A_MN ? wgmma_desc_sw128(sr + kk * 2048, 8192, 1024) : wgmma_desc_sw128(sr + kk * 32, 16, 1024);
+        if constexpr (FP8) WgmmaFp8SS<BLOCK_N, AE5, BE5>::mma(acc[r], da, db, (i > 0 || kk > 0) ? 1 : 0);
+        else WgmmaBf16SS<BLOCK_N, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc[r], da, db, (i > 0 || kk > 0) ? 1 : 0);
+      }
     }
     wgmma_commit();
     wgmma_wait<1>();                              // the group that read slot `prev` has retired
@@ -224,102 +254,25 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[BLOCK_N / 2], uin
     prev = s;
     if (++s == C::STAGES) { s = 0; ph ^= 1; }
   }
+  if (arrive_bar >= 0) asm volatile("bar.arrive %0, 256;" ::"r"(arrive_bar) : "memory");
   wgmma_wait<0>();
-  wgmma_fence_regs(acc);
+#pragma unroll
+  for (int r = 0; r < R; ++r) wgmma_fence_regs(acc[r]);
   if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 }
 
-template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const GemmArgs p) {
-  using C = Cfg<BLOCK_N>;
-  static_assert(!FP8 || (!A_MN && !B_MN), "fp8 wgmma reads K-major operands only");
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C::STAGES;
-
-  const int wg = threadIdx.x >> 7;
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);               // one arrival per consumer warp
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-  pdl_wait();
-  pdl_trigger();
-
-  const int tile = blockIdx.x;
-  const int nb = tile % p.n_blocks;
-  const int mb = (tile / p.n_blocks) % p.m_blocks;
-  const int ks = tile / (p.n_blocks * p.m_blocks);
-  const int kb0 = ks * p.k_per_split;
-  const int kb1 = min(p.k_blocks, kb0 + p.k_per_split);
-  constexpr int BK = FP8 ? 128 : 64;             // elements along K per stage
-
-  if (wg == 0) {
-    // ------------------------------------------------------------------ TMA producer
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
-    if (threadIdx.x == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait_mma(&empty_bar[s], ph ^ 1);
-        uint8_t* sa = smem + s * C::STAGE_BYTES;
-        uint8_t* sb = sa + C::A_BYTES;
-        mbar_arrive_expect_tx(&full_bar[s], C::STAGE_BYTES);
-        if constexpr (!A_MN) {
-          tma_load_2d(sa, &tmap_a, &full_bar[s], kb * BK, mb * BLOCK_M);
-        } else {
-#pragma unroll
-          for (int j = 0; j < BLOCK_M / 64; ++j)
-            tma_load_2d(sa + j * 8192, &tmap_a, &full_bar[s], mb * BLOCK_M + j * 64, kb * BK);
-        }
-        if constexpr (!B_MN) {
-          tma_load_2d(sb, &tmap_b, &full_bar[s], kb * BK, nb * BLOCK_N);
-        } else {
-#pragma unroll
-          for (int j = 0; j < BLOCK_N / 64; ++j)
-            tma_load_2d(sb + j * 8192, &tmap_b, &full_bar[s], nb * BLOCK_N + j * 64, kb * BK);
-        }
-        if (++s == C::STAGES) { s = 0; ph ^= 1; }
-      }
-    }
-    return;
-  }
-  // -------------------------------------------------------------------- MMA + epilogue (two warpgroups x 64 rows)
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
-  const int cw = wg - 1;
-  float acc[BLOCK_N / 2];                       // the first MMA of the tile overwrites it (scale-d = 0)
-  const int nkb = kb1 - kb0;
-  if constexpr (FP8) {
-    switch (p.fp8_fmt & 3u) {
-      case 0: consumer_mainloop<A_MN, B_MN, BLOCK_N, true, 0, 0>(acc, smem, full_bar, empty_bar, cw, nkb); break;
-      case 1: consumer_mainloop<A_MN, B_MN, BLOCK_N, true, 1, 0>(acc, smem, full_bar, empty_bar, cw, nkb); break;
-      case 2: consumer_mainloop<A_MN, B_MN, BLOCK_N, true, 0, 1>(acc, smem, full_bar, empty_bar, cw, nkb); break;
-      default: consumer_mainloop<A_MN, B_MN, BLOCK_N, true, 1, 1>(acc, smem, full_bar, empty_bar, cw, nkb); break;
-    }
-  } else {
-    consumer_mainloop<A_MN, B_MN, BLOCK_N, false, 0, 0>(acc, smem, full_bar, empty_bar, cw, nkb);
-  }
-  if (nkb <= 0) return;
-
-  float alpha = p.alpha;
-  if constexpr (FP8) alpha *= __ldg(p.scale_a) * __ldg(p.scale_b);   // per-tensor dequantisation
-  const unsigned long long seed = p.drop_thresh16 != 0 ? p.seed.value() : 0ull;
+// Epilogue of one warpgroup's 64 x NCOLS accumulator fragment: output rows [row64, row64 + 64), columns from col0.
+template <int NCOLS>
+__device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc)[NCOLS / 2], int row64, int col0,
+                                                  float alpha, unsigned long long seed, bool add_local) {
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const int c = lane & 3;
-  const int row_base = mb * BLOCK_M + cw * 64 + warp * 16 + (lane >> 2);
+  const int row_base = row64 + warp * 16 + (lane >> 2);
   const bool bf16_out = p.epi != EPI_ACCUM_F32 && p.epi != EPI_F32;
 #pragma unroll
-  for (int i = 0; i < BLOCK_N / 32; ++i) {         // unrolled: the accumulator must stay in registers
-    const int n0 = nb * BLOCK_N + i * 32 + c * 8;            // after the regrouping this lane owns columns [n0, n0 + 8)
-    if (nb * BLOCK_N + i * 32 >= p.N) break;                 // warp uniform
+  for (int i = 0; i < NCOLS / 32; ++i) {           // unrolled: the accumulator must stay in registers
+    const int n0 = col0 + i * 32 + c * 8;                    // after the regrouping this lane owns columns [n0, n0 + 8)
+    if (col0 + i * 32 >= p.N) break;                         // warp uniform
     float cs[8];
 #pragma unroll
     for (int t = 0; t < 8; ++t) cs[t] = 0.f;
@@ -341,7 +294,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           f[2 * k] = __uint_as_float(lo[k]) * alpha;
           f[2 * k + 1] = __uint_as_float(hi[k]) * alpha;
         }
-        epilogue_group(p, f, row, n0, seed, ks == 0);
+        epilogue_group(p, f, row, n0, seed, add_local);
 #pragma unroll
         for (int t = 0; t < 8; ++t) cs[t] += f[t];
       }
@@ -358,6 +311,114 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         for (int t = 0; t < 8; ++t) atomicAdd(p.colsum + n0 + t, cs[t]);
       }
     }
+  }
+}
+
+// The consumer warpgroup `cw` (0 or 1) over this CTA's units.  Ping-pong (BLOCK_N 128): warpgroup cw takes the
+// CTA's units j = cw, cw + 2, ...; it waits on named barrier 1 + cw for its turn to issue MMAs and, if the other
+// warpgroup has a next unit, hands the turn over on barrier 2 - cw once its own MMAs are issued.  The order also keeps
+// a warpgroup from running more than one ring phase ahead of the producer.
+template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int AE5, int BE5>
+__device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                         int cw) {
+  constexpr bool PINGPONG = BLOCK_N == 128;
+  constexpr int R = PINGPONG ? 2 : 1;            // 64-row accumulator fragments per warpgroup
+  float acc[R][BLOCK_N / 2];                     // the first MMA of a unit overwrites it (scale-d = 0)
+  float alpha = p.alpha;
+  if constexpr (FP8) alpha *= __ldg(p.scale_a) * __ldg(p.scale_b);   // per-tensor dequantisation
+  const unsigned long long seed = p.drop_thresh16 != 0 ? p.seed.value() : 0ull;
+  if (PINGPONG && cw == 1) asm volatile("bar.arrive 1, 256;" ::: "memory");   // warpgroup 0 goes first
+  uint32_t it = 0;                               // ring position of the unit: k-blocks of this CTA's earlier units
+  int j = 0;
+  for (int u = blockIdx.x; u < p.units; u += gridDim.x, ++j) {
+    const Unit w = unit_of(p, u);
+    if (PINGPONG && (j & 1) != cw) {
+      it += w.nkb;
+      continue;
+    }
+    if (PINGPONG) asm volatile("bar.sync %0, 256;" ::"r"(1 + cw) : "memory");
+    const int arrive_bar = PINGPONG && u + (int)gridDim.x < p.units ? 2 - cw : -1;
+    consumer_mainloop<A_MN, B_MN, BLOCK_N, R, FP8, AE5, BE5>(acc, smem, full_bar, empty_bar, PINGPONG ? 0 : cw, it,
+                                                            w.nkb, arrive_bar);
+    it += w.nkb;
+    const int row64 = w.mb * BLOCK_M + (PINGPONG ? 0 : cw * 64);
+#pragma unroll
+    for (int r = 0; r < R; ++r)
+      fragment_epilogue<BLOCK_N>(p, acc[r], row64 + r * 64, w.nb * BLOCK_N, alpha, seed, w.ks == 0);
+  }
+}
+
+template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const GemmArgs p) {
+  using C = Cfg<BLOCK_N>;
+  static_assert(!FP8 || (!A_MN && !B_MN), "fp8 wgmma reads K-major operands only");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + C::STAGES;
+
+  const int wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int s = 0; s < C::STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], BLOCK_N == 128 ? 4 : 8);   // one arrival per warp of the warpgroup(s) reading the slot
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_trigger();
+  constexpr int BK = FP8 ? 128 : 64;             // elements along K per stage
+
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      int s = 0;
+      uint32_t ph = 0;
+      for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+        const Unit w = unit_of(p, u);
+        for (int kb = w.kb0; kb < w.kb0 + w.nkb; ++kb) {
+          mbar_wait_mma(&empty_bar[s], ph ^ 1);
+          uint8_t* sa = smem + s * C::STAGE_BYTES;
+          uint8_t* sb = sa + C::A_BYTES;
+          mbar_arrive_expect_tx(&full_bar[s], C::STAGE_BYTES);
+          if constexpr (!A_MN) {
+            tma_load_2d(sa, &tmap_a, &full_bar[s], kb * BK, w.mb * BLOCK_M);
+          } else {
+#pragma unroll
+            for (int j = 0; j < BLOCK_M / 64; ++j)
+              tma_load_2d(sa + j * 8192, &tmap_a, &full_bar[s], w.mb * BLOCK_M + j * 64, kb * BK);
+          }
+          if constexpr (!B_MN) {
+            tma_load_2d(sb, &tmap_b, &full_bar[s], kb * BK, w.nb * BLOCK_N);
+          } else {
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 64; ++j)
+              tma_load_2d(sb + j * 8192, &tmap_b, &full_bar[s], w.nb * BLOCK_N + j * 64, kb * BK);
+          }
+          if (++s == C::STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+  // -------------------------------------------------------------------- MMA + epilogue (two warpgroups)
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = wg - 1;
+  if constexpr (FP8) {
+    switch (p.fp8_fmt & 3u) {
+      case 0: consumer<A_MN, B_MN, BLOCK_N, true, 0, 0>(p, smem, full_bar, empty_bar, cw); break;
+      case 1: consumer<A_MN, B_MN, BLOCK_N, true, 1, 0>(p, smem, full_bar, empty_bar, cw); break;
+      case 2: consumer<A_MN, B_MN, BLOCK_N, true, 0, 1>(p, smem, full_bar, empty_bar, cw); break;
+      default: consumer<A_MN, B_MN, BLOCK_N, true, 1, 1>(p, smem, full_bar, empty_bar, cw); break;
+    }
+  } else {
+    consumer<A_MN, B_MN, BLOCK_N, false, 0, 0>(p, smem, full_bar, empty_bar, cw);
   }
 }
 
@@ -503,7 +564,8 @@ static void launch(const GemmCall& c, cudaStream_t st) {
     B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_TOTAL));
     configured = true;
   }
-  const int grid = p.m_blocks * p.n_blocks * p.k_splits;
+  p.units = p.m_blocks * p.n_blocks * p.k_splits;
+  const int grid = p.units < num_sms() ? p.units : num_sms();       // persistent: one CTA per SM walks the units
   launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_TOTAL, st, ta, tb, p);
 }
 

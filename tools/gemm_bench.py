@@ -1,5 +1,10 @@
-"""Device-timed throughput of the wgmma GEMM on the BERT-large shapes vs torch.matmul (cuBLAS) ->
-gpurun_out/gemm_bench.json.  CUDA events, warm-up, L2 flush between iterations."""
+"""Device-timed throughput of the wgmma GEMM on the BERT-large shapes vs torch.matmul (cuBLAS), printed as one JSON
+line per shape.  CUDA events, warm-up, L2 flush between iterations.
+
+    python tools/gemm_bench.py [--epi] [--fp8] [--only NAME]
+
+``--epi`` also times every shape with the epilogue the fused engine runs on it (wgrad: ``wgrad_accumulate``, the
+split-K factor the engine picks)."""
 import json
 import os
 import sys
@@ -26,15 +31,42 @@ def timeit(fn, iters=20, warm=5):
     return ts[len(ts) // 2]
 
 
+M = 12288          # phase 1: micro-batch 96 x seq 128
+# (name, layout, M, N, K, engine epilogue): every GEMM of one encoder layer, then the MLM decoder and a square check
+SHAPES = [("qkv_fwd", K.NT, M, 3072, 1024, "bias"), ("attn_out_fwd", K.NT, M, 1024, 1024, "bias_drop_res"),
+          ("ffn1_fwd", K.NT, M, 4096, 1024, "bias_gelu_dg"), ("ffn2_fwd", K.NT, M, 1024, 4096, "bias_drop_res"),
+          ("ffn2_dgrad", K.NN, M, 4096, 1024, "mul_colsum"), ("ffn1_dgrad", K.NN, M, 1024, 4096, "add"),
+          ("attn_out_dgrad", K.NN, M, 1024, 1024, "none"), ("qkv_dgrad", K.NN, M, 1024, 3072, "add"),
+          ("ffn2_wgrad", K.TN, 1024, 4096, M, "wgrad"), ("ffn1_wgrad", K.TN, 4096, 1024, M, "wgrad"),
+          ("attn_out_wgrad", K.TN, 1024, 1024, M, "wgrad"), ("qkv_wgrad", K.TN, 3072, 1024, M, "wgrad"),
+          ("decoder_fwd", K.NT, 1920, 30528, 1024, "bias"), ("big", K.NT, 8192, 8192, 8192, "none")]
+
+
+def engine_call(a, b, layout, m, n, epi, block_n=None):
+    """the GEMM call the fused engine makes on this shape, with its fused epilogue (``block_n``: force a tile width)"""
+    if epi == "wgrad":
+        g = torch.zeros(m, n, device="cuda")
+        return lambda: K.wgrad_accumulate(a, b, g)
+    o = torch.empty(m, n, device="cuda", dtype=torch.bfloat16)
+    kw = dict(layout=layout, out=o, block_n=block_n)
+    if epi == "bias":
+        kw.update(epi=K.EPI_BIAS, bias=torch.randn(n, device="cuda").bfloat16())
+    elif epi == "bias_gelu_dg":
+        kw.update(epi=K.EPI_BIAS_GELU_DG, bias=torch.randn(n, device="cuda").bfloat16(), aux_out=torch.empty_like(o))
+    elif epi == "bias_drop_res":
+        kw.update(epi=K.EPI_BIAS_DROP_RES, bias=torch.randn(n, device="cuda").bfloat16(),
+                  res=torch.randn(m, n, device="cuda").bfloat16(), p_drop=0.1,
+                  mask_in=K.dropout_mask(m, n, 0.1, 1, 3, "cuda"))
+    elif epi == "mul_colsum":
+        kw.update(epi=K.EPI_MUL, res=torch.randn(m, n, device="cuda").bfloat16(), colsum=torch.zeros(n, device="cuda"))
+    elif epi == "add":
+        kw.update(epi=K.EPI_ADD, res=torch.randn(m, n, device="cuda").bfloat16())
+    return lambda: K.gemm(a, b, **kw)
+
+
 def main():
     only = sys.argv[sys.argv.index("--only") + 1] if "--only" in sys.argv else None
-    M = 12288
-    out = []
-    shapes = [("qkv_fwd", K.NT, M, 3072, 1024), ("attn_out_fwd", K.NT, M, 1024, 1024), ("ffn1_fwd", K.NT, M, 4096, 1024),
-              ("ffn2_fwd", K.NT, M, 1024, 4096), ("ffn1_dgrad", K.NN, M, 1024, 4096), ("ffn2_dgrad", K.NN, M, 4096, 1024),
-              ("ffn1_wgrad", K.TN, 4096, 1024, M), ("ffn2_wgrad", K.TN, 1024, 4096, M), ("qkv_wgrad", K.TN, 3072, 1024, M),
-              ("decoder_fwd", K.NT, 1920, 30528, 1024), ("big", K.NT, 8192, 8192, 8192)]
-    for name, layout, m, n, k in shapes:
+    for name, layout, m, n, k, epi in SHAPES:
         if only is not None and name != only:
             continue
         if layout == K.NT:
@@ -60,6 +92,13 @@ def main():
                 o = torch.empty(m, n, device="cuda", dtype=torch.bfloat16)
                 t = timeit(lambda: K.gemm(a, b, layout=layout, out=o, block_n=bn))
                 rec[f"ours_bn{bn}_ms"], rec[f"ours_bn{bn}_tflops"] = round(t, 4), round(flops / t / 1e9, 1)
+        if "--epi" in sys.argv:
+            t = timeit(engine_call(a, b, layout, m, n, epi))
+            rec[f"engine_{epi}_ms"], rec[f"engine_{epi}_tflops"] = round(t, 4), round(flops / t / 1e9, 1)
+            if layout != K.TN:
+                for bn in (128, 256):
+                    t = timeit(engine_call(a, b, layout, m, n, epi, bn))
+                    rec[f"engine_{epi}_bn{bn}_tflops"] = round(flops / t / 1e9, 1)
         if "--fp8" in sys.argv:          # same shape with e4m3 (e5m2 for the gradient operand) bytes
             a_e5 = layout != K.NT
             meta = K.Fp8Meta(["a", "b"], [a_e5, False], "cuda")
@@ -69,34 +108,13 @@ def main():
                 o = torch.zeros(m, n, device="cuda")
                 for sp in (1, 2, 4, -1):
                     t = timeit(lambda: K.gemm(qa, qb, epi=K.EPI_ACCUM_F32, out=o, k_splits=sp, **kw))
-                    rec[f"fp8_s{'treamk' if sp < 0 else sp}_tflops"] = round(flops / t / 1e9, 1)
+                    rec[f"fp8_s{'auto' if sp < 0 else sp}_tflops"] = round(flops / t / 1e9, 1)
             else:
                 o = torch.empty(m, n, device="cuda", dtype=torch.bfloat16)
                 t = timeit(lambda: K.gemm(qa, qb, out=o, **kw))
                 rec["fp8_ms"], rec["fp8_tflops"] = round(t, 4), round(flops / t / 1e9, 1)
             t = timeit(lambda: meta.quantize(a, "a", out=qa))
             rec["quantize_a_gbs"] = round(a.numel() * 3 / t / 1e6, 1)
-        if "--epi" in sys.argv and name in ("ffn1_fwd", "ffn2_dgrad", "attn_out_fwd", "ffn2_fwd"):
-            # the fused epilogues the engine runs on this shape, against the plain bf16 store
-            o = torch.empty(m, n, device="cuda", dtype=torch.bfloat16)
-            if name == "ffn1_fwd":
-                bias, aux = torch.randn(n, device="cuda").bfloat16(), torch.empty_like(o)
-                t = timeit(lambda: K.gemm(a, b, layout=layout, out=o, epi=K.EPI_BIAS_GELU_DG, bias=bias, aux_out=aux))
-                rec["epi_bias_gelu_dg_tflops"] = round(flops / t / 1e9, 1)
-                t = timeit(lambda: K.gemm(a, b, layout=layout, out=o, epi=K.EPI_BIAS, bias=bias))
-                rec["epi_bias_tflops"] = round(flops / t / 1e9, 1)
-            elif name == "ffn2_dgrad":
-                res, cs = torch.randn(m, n, device="cuda").bfloat16(), torch.zeros(n, device="cuda")
-                t = timeit(lambda: K.gemm(a, b, layout=layout, out=o, epi=K.EPI_MUL, res=res, colsum=cs))
-                rec["epi_mul_colsum_tflops"] = round(flops / t / 1e9, 1)
-                t = timeit(lambda: K.gemm(a, b, layout=layout, out=o, epi=K.EPI_MUL, res=res))
-                rec["epi_mul_tflops"] = round(flops / t / 1e9, 1)
-            else:
-                bias, res = torch.randn(n, device="cuda").bfloat16(), torch.randn(m, n, device="cuda").bfloat16()
-                t = timeit(lambda: K.gemm(a, b, layout=layout, out=o, epi=K.EPI_BIAS_DROP_RES, bias=bias, res=res, p_drop=0.1,
-                                          seed=1, stream=3))
-                rec["epi_bias_drop_res_tflops"] = round(flops / t / 1e9, 1)
-        out.append(rec)
         print(json.dumps(rec), flush=True)
 
 
