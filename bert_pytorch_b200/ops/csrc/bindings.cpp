@@ -179,7 +179,15 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
   b200::gemm_bf16(c, cur_stream());
 }
 
-void layer_norm_fwd(Tensor x, Tensor gamma, Tensor beta, Tensor y, c10::optional<Tensor> mean,
+// In-kernel GEMM timeline (tools/gemm_timeline.py): `buf` is int64 [units, 16]; None turns recording off.
+bool gemm_timeline(c10::optional<Tensor> buf) {
+  if (!buf.has_value() || !buf->defined()) return b200::gemm_set_timeline(nullptr, 0);
+  TORCH_CHECK(buf->is_cuda() && buf->scalar_type() == at::kLong && buf->is_contiguous() && buf->dim() == 2 &&
+              buf->size(1) == 16, "gemm_timeline: int64 CUDA tensor [units, 16]");
+  return b200::gemm_set_timeline(reinterpret_cast<long long*>(buf->data_ptr<int64_t>()), buf->size(0));
+}
+
+void layer_norm_fwd(Tensor x,Tensor gamma, Tensor beta, Tensor y, c10::optional<Tensor> mean,
                     c10::optional<Tensor> rstd, double eps, double p_drop, int64_t seed, int64_t stream_id,
                     c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2) {
   check_bf16(x, "x"); check_bf16(y, "y");
@@ -488,6 +496,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("dropout_mask", &dropout_mask);
   m.doc() = "bert_pytorch_b200 sm_90a kernels";
   m.def("gemm", &gemm);
+  m.def("gemm_timeline", &gemm_timeline);
   m.def("set_seed_step", &set_seed_step);
   m.def("set_grad_peers", &set_grad_peers);
   m.def("set_grad_push", &set_grad_push);

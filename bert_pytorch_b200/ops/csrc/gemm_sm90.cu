@@ -81,14 +81,37 @@ struct GemmArgs {
   long long peer_off;        // element offset of `out` inside the arena
   long long peer_per;        // shard size in elements: owner(e) = min(e / peer_per, world - 1)
   float* peer_base[16];      // gradient arena of every rank (symmetric-memory mapping)
+#ifdef B200_GEMM_TIMELINE
+  long long* timeline;       // [units][TL_STRIDE] clock64 stamps (nullptr: not recorded), see gemm_set_timeline
+#endif
 };
+
+// In-kernel timeline (build with -DB200_GEMM_TIMELINE, read by tools/gemm_timeline.py).  Record of unit u:
+//   [6 cw + 0..5]  consumer warpgroup cw that ran the unit: turn taken, first full_bar passed, last MMA issued,
+//                  wgmma_wait<0> returned, epilogue done, cycles spent waiting on full_bar
+//   [12] cycles the producer was blocked on empty_bar while loading the unit   [13] gridDim.x
+// SM clock cycles (clock64): stamps are compared only within one CTA.  Register reads only, so the define adds no
+// call to the wgmma pipeline.
+#ifdef B200_GEMM_TIMELINE
+constexpr int TL_STRIDE = 16;
+struct UnitStamps {
+  long long start, full0, last_mma, wait0, epi_done, op_wait;
+};
+#define TL(...) __VA_ARGS__
+#else
+#define TL(...)
+#endif
 
 // Epilogue of 8 consecutive output columns [n0, n0 + 8) of one row (n0 % 8 == 0, N % 8 == 0).  `f` holds
 // alpha * accumulator.  Returns through `f` the values that were stored (bf16-rounded) for the column sums.
+// E >= 0: the epilogue is fixed at compile time (must equal p.epi), so a kernel carries the code of that epilogue
+// alone; E < 0: chosen at run time from p.epi.
+template <int E>
 __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8], int row, int n0, unsigned long long seed,
                                                bool add_local) {
+  const int epi = E >= 0 ? E : p.epi;
   const size_t ooff = (size_t)row * p.ldo + n0;
-  if (p.epi == EPI_ACCUM_F32) {
+  if (epi == EPI_ACCUM_F32) {
     float* o = reinterpret_cast<float*>(p.out) + ooff;
     if (p.peer_world > 1) {
       // an 8-column group crosses at most one shard boundary (shards are multiples of 2048 elements)
@@ -121,14 +144,14 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
                    "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
     return;
   }
-  if (p.epi == EPI_F32) {
+  if (epi == EPI_F32) {
     float* o = reinterpret_cast<float*>(p.out) + ooff;
     *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
     *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
     return;
   }
-  if (p.bias != nullptr && (p.epi == EPI_BIAS || p.epi == EPI_BIAS_GELU || p.epi == EPI_BIAS_DROP_RES ||
-                            p.epi == EPI_BIAS_TANH || p.epi == EPI_BIAS_GELU_DG)) {
+  if (p.bias != nullptr && (epi == EPI_BIAS || epi == EPI_BIAS_GELU || epi == EPI_BIAS_DROP_RES ||
+                            epi == EPI_BIAS_TANH || epi == EPI_BIAS_GELU_DG)) {
     const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + n0));
     const uint32_t w[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
@@ -138,12 +161,12 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
       f[2 * t + 1] += bb.y;
     }
   }
-  if (p.epi == EPI_BIAS_GELU) {                  // save the pre-activation, then activate
+  if (epi == EPI_BIAS_GELU) {                  // save the pre-activation, then activate
     *reinterpret_cast<uint4*>(p.aux_out + ooff) =
         make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
 #pragma unroll
     for (int j = 0; j < 8; ++j) f[j] = gelu_erf(f[j]);
-  } else if (p.epi == EPI_BIAS_GELU_DG) {
+  } else if (epi == EPI_BIAS_GELU_DG) {
     float dg[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -153,11 +176,11 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
     }
     *reinterpret_cast<uint4*>(p.aux_out + ooff) =
         make_uint4(pack_bf16(dg[0], dg[1]), pack_bf16(dg[2], dg[3]), pack_bf16(dg[4], dg[5]), pack_bf16(dg[6], dg[7]));
-  } else if (p.epi == EPI_BIAS_TANH) {
+  } else if (epi == EPI_BIAS_TANH) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) f[j] = tanhf(f[j]);
-  } else if (p.epi == EPI_BIAS_DROP_RES || p.epi == EPI_ADD || p.epi == EPI_DGELU || p.epi == EPI_MUL) {
-    if (p.epi == EPI_BIAS_DROP_RES && p.drop_thresh16 != 0) {
+  } else if (epi == EPI_BIAS_DROP_RES || epi == EPI_ADD || epi == EPI_DGELU || epi == EPI_MUL) {
+    if (epi == EPI_BIAS_DROP_RES && p.drop_thresh16 != 0) {
       const size_t moff = (size_t)row * (size_t)(p.N >> 3) + (size_t)(n0 >> 3);
       uint32_t kb;
       if (p.mask_in != nullptr) {
@@ -171,7 +194,7 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
         if (p.mask_out != nullptr) p.mask_out[moff] = (unsigned char)kb;
       }
 #pragma unroll
-      for (int t = 0; t < 8; ++t) f[t] = (kb >> t) & 1u ? f[t] * p.drop_scale : 0.f;
+      for (int t = 0; t < 8; ++t) f[t] = (kb >> t) & 1u ? __fmul_rn(f[t], p.drop_scale) : 0.f;
     }
     if (p.res != nullptr) {
       const uint4 r = *reinterpret_cast<const uint4*>(p.res + (size_t)row * p.ldr + n0);
@@ -179,10 +202,10 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
         const float2 rr = unpack_bf16(w[t]);
-        if (p.epi == EPI_DGELU) {
+        if (epi == EPI_DGELU) {
           f[2 * t] *= dgelu_erf(rr.x);
           f[2 * t + 1] *= dgelu_erf(rr.y);
-        } else if (p.epi == EPI_MUL) {
+        } else if (epi == EPI_MUL) {
           f[2 * t] *= rr.x;
           f[2 * t + 1] *= rr.y;
         } else {
@@ -224,7 +247,7 @@ __device__ __forceinline__ Unit unit_of(const GemmArgs& p, int u) {
 template <bool A_MN, bool B_MN, int BLOCK_N, int R, bool FP8, int AE5, int BE5>
 __device__ __forceinline__ void consumer_mainloop(float (&acc)[R][BLOCK_N / 2], uint8_t* smem, uint64_t* full_bar,
                                                   uint64_t* empty_bar, int a_chunk, uint32_t it, int nkb,
-                                                  int arrive_bar) {
+                                                  int arrive_bar TL(, UnitStamps& st)) {
   using C = Cfg<BLOCK_N>;
   const int lane = threadIdx.x & 31;
   int s = it % C::STAGES, prev = -1;
@@ -232,7 +255,16 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[R][BLOCK_N / 2], 
 #pragma unroll
   for (int r = 0; r < R; ++r) wgmma_fence_regs(acc[r]);
   for (int i = 0; i < nkb; ++i) {
+#ifdef B200_GEMM_TIMELINE
+    if (!mbar_try_wait(&full_bar[s], ph)) {
+      const long long t = clock64();
+      mbar_wait_mma(&full_bar[s], ph);
+      st.op_wait += clock64() - t;
+    }
+    if (i == 0) st.full0 = clock64();
+#else
     mbar_wait_mma(&full_bar[s], ph);
+#endif
     const uint32_t sa = smem_u32(smem + s * C::STAGE_BYTES) + a_chunk * 8192;   // 64 rows (or a 64-wide MN chunk) of A
     const uint32_t sb = smem_u32(smem + s * C::STAGE_BYTES) + C::A_BYTES;
     wgmma_fence();
@@ -249,6 +281,7 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[R][BLOCK_N / 2], 
       }
     }
     wgmma_commit();
+    TL(st.last_mma = clock64();)
     wgmma_wait<1>();                              // the group that read slot `prev` has retired
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
     prev = s;
@@ -258,17 +291,19 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[R][BLOCK_N / 2], 
   wgmma_wait<0>();
 #pragma unroll
   for (int r = 0; r < R; ++r) wgmma_fence_regs(acc[r]);
+  TL(st.wait0 = clock64();)
   if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 }
 
 // Epilogue of one warpgroup's 64 x NCOLS accumulator fragment: output rows [row64, row64 + 64), columns from col0.
-template <int NCOLS>
+template <int NCOLS, int E>
 __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc)[NCOLS / 2], int row64, int col0,
                                                   float alpha, unsigned long long seed, bool add_local) {
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const int c = lane & 3;
   const int row_base = row64 + warp * 16 + (lane >> 2);
-  const bool bf16_out = p.epi != EPI_ACCUM_F32 && p.epi != EPI_F32;
+  const int epi = E >= 0 ? E : p.epi;
+  const bool bf16_out = epi != EPI_ACCUM_F32 && epi != EPI_F32;
 #pragma unroll
   for (int i = 0; i < NCOLS / 32; ++i) {           // unrolled: the accumulator must stay in registers
     const int n0 = col0 + i * 32 + c * 8;                    // after the regrouping this lane owns columns [n0, n0 + 8)
@@ -291,10 +326,12 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
         float f[8];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          f[2 * k] = __uint_as_float(lo[k]) * alpha;
-          f[2 * k + 1] = __uint_as_float(hi[k]) * alpha;
+          // __fmul_rn: never contracted with the bias or residual add that follows (the same rounding as when the
+          // epilogue is chosen at run time and a branch separates the two)
+          f[2 * k] = __fmul_rn(__uint_as_float(lo[k]), alpha);
+          f[2 * k + 1] = __fmul_rn(__uint_as_float(hi[k]), alpha);
         }
-        epilogue_group(p, f, row, n0, seed, add_local);
+        epilogue_group<E>(p, f, row, n0, seed, add_local);
 #pragma unroll
         for (int t = 0; t < 8; ++t) cs[t] += f[t];
       }
@@ -318,7 +355,7 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
 // CTA's units j = cw, cw + 2, ...; it waits on named barrier 1 + cw for its turn to issue MMAs and, if the other
 // warpgroup has a next unit, hands the turn over on barrier 2 - cw once its own MMAs are issued.  The order also keeps
 // a warpgroup from running more than one ring phase ahead of the producer.
-template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int AE5, int BE5>
+template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int AE5, int BE5, int E>
 __device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                          int cw) {
   constexpr bool PINGPONG = BLOCK_N == 128;
@@ -337,18 +374,28 @@ __device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint6
       continue;
     }
     if (PINGPONG) asm volatile("bar.sync %0, 256;" ::"r"(1 + cw) : "memory");
+    TL(UnitStamps st{}; st.start = clock64();)
     const int arrive_bar = PINGPONG && u + (int)gridDim.x < p.units ? 2 - cw : -1;
     consumer_mainloop<A_MN, B_MN, BLOCK_N, R, FP8, AE5, BE5>(acc, smem, full_bar, empty_bar, PINGPONG ? 0 : cw, it,
-                                                            w.nkb, arrive_bar);
+                                                            w.nkb, arrive_bar TL(, st));
     it += w.nkb;
     const int row64 = w.mb * BLOCK_M + (PINGPONG ? 0 : cw * 64);
 #pragma unroll
     for (int r = 0; r < R; ++r)
-      fragment_epilogue<BLOCK_N>(p, acc[r], row64 + r * 64, w.nb * BLOCK_N, alpha, seed, w.ks == 0);
+      fragment_epilogue<BLOCK_N, E>(p, acc[r], row64 + r * 64, w.nb * BLOCK_N, alpha, seed, w.ks == 0);
+#ifdef B200_GEMM_TIMELINE
+    st.epi_done = clock64();
+    if (p.timeline != nullptr && (threadIdx.x & 127) == 0) {
+      long long* rec = p.timeline + (size_t)u * TL_STRIDE + cw * 6;
+      rec[0] = st.start; rec[1] = st.full0; rec[2] = st.last_mma; rec[3] = st.wait0; rec[4] = st.epi_done;
+      rec[5] = st.op_wait;
+    }
+#endif
   }
 }
 
-template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8>
+// E: the epilogue, fixed at compile time (>= 0) or read from p.epi (< 0), see epilogue_group
+template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int E>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const GemmArgs p) {
@@ -382,8 +429,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       uint32_t ph = 0;
       for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
         const Unit w = unit_of(p, u);
+        TL(long long blocked = 0;)
         for (int kb = w.kb0; kb < w.kb0 + w.nkb; ++kb) {
+          TL(const long long t = clock64();)
           mbar_wait_mma(&empty_bar[s], ph ^ 1);
+          TL(blocked += clock64() - t;)
           uint8_t* sa = smem + s * C::STAGE_BYTES;
           uint8_t* sb = sa + C::A_BYTES;
           mbar_arrive_expect_tx(&full_bar[s], C::STAGE_BYTES);
@@ -403,6 +453,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           }
           if (++s == C::STAGES) { s = 0; ph ^= 1; }
         }
+#ifdef B200_GEMM_TIMELINE
+        if (p.timeline != nullptr) {
+          p.timeline[(size_t)u * TL_STRIDE + 12] = blocked;
+          p.timeline[(size_t)u * TL_STRIDE + 13] = gridDim.x;
+        }
+#endif
       }
     }
     return;
@@ -412,13 +468,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int cw = wg - 1;
   if constexpr (FP8) {
     switch (p.fp8_fmt & 3u) {
-      case 0: consumer<A_MN, B_MN, BLOCK_N, true, 0, 0>(p, smem, full_bar, empty_bar, cw); break;
-      case 1: consumer<A_MN, B_MN, BLOCK_N, true, 1, 0>(p, smem, full_bar, empty_bar, cw); break;
-      case 2: consumer<A_MN, B_MN, BLOCK_N, true, 0, 1>(p, smem, full_bar, empty_bar, cw); break;
-      default: consumer<A_MN, B_MN, BLOCK_N, true, 1, 1>(p, smem, full_bar, empty_bar, cw); break;
+      case 0: consumer<A_MN, B_MN, BLOCK_N, true, 0, 0, E>(p, smem, full_bar, empty_bar, cw); break;
+      case 1: consumer<A_MN, B_MN, BLOCK_N, true, 1, 0, E>(p, smem, full_bar, empty_bar, cw); break;
+      case 2: consumer<A_MN, B_MN, BLOCK_N, true, 0, 1, E>(p, smem, full_bar, empty_bar, cw); break;
+      default: consumer<A_MN, B_MN, BLOCK_N, true, 1, 1, E>(p, smem, full_bar, empty_bar, cw); break;
     }
   } else {
-    consumer<A_MN, B_MN, BLOCK_N, false, 0, 0>(p, smem, full_bar, empty_bar, cw);
+    consumer<A_MN, B_MN, BLOCK_N, false, 0, 0, E>(p, smem, full_bar, empty_bar, cw);
   }
 }
 
@@ -519,7 +575,20 @@ CUtensorMap make_tmap_2d_u8(const void* ptr, uint64_t inner, uint64_t outer, uin
 }
 
 
-template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8>
+static long long* g_timeline = nullptr;
+static long long g_timeline_units = 0;
+
+bool gemm_set_timeline(long long* buf, long long units) {
+  g_timeline = buf;
+  g_timeline_units = buf != nullptr ? units : 0;
+#ifdef B200_GEMM_TIMELINE
+  return true;
+#else
+  return false;
+#endif
+}
+
+template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int E = -1>
 static void launch(const GemmCall& c, cudaStream_t st) {
   using C = Cfg<BLOCK_N>;
   constexpr int BK = FP8 ? 128 : 64;
@@ -558,13 +627,16 @@ static void launch(const GemmCall& c, cudaStream_t st) {
                         : make_tmap_2d(c.A, c.K, c.M, c.lda, BK, 64 * 2, ES);
   CUtensorMap tb = B_MN ? make_tmap_2d(c.B, c.N, c.K, c.ldb, 64, BK, ES)
                         : make_tmap_2d(c.B, c.K, c.N, c.ldb, BK, BLOCK_N, ES);
-  auto kern = gemm_kernel<A_MN, B_MN, BLOCK_N, FP8>;
+  auto kern = gemm_kernel<A_MN, B_MN, BLOCK_N, FP8, E>;
   static bool configured = false;
   if (!configured) {
     B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_TOTAL));
     configured = true;
   }
   p.units = p.m_blocks * p.n_blocks * p.k_splits;
+#ifdef B200_GEMM_TIMELINE
+  p.timeline = p.units <= g_timeline_units ? g_timeline : nullptr;
+#endif
   const int grid = p.units < num_sms() ? p.units : num_sms();       // persistent: one CTA per SM walks the units
   launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_TOTAL, st, ta, tb, p);
 }
@@ -577,6 +649,12 @@ static const void* fp8_k_major(const void* src, int mn, int K, int ld, int* ld_o
   fp8_transpose_kernel<<<dim3((mn + 63) / 64, (K + 63) / 64), 256, 0, st>>>((const uint8_t*)src, (uint8_t*)buf, K, mn, ld, Kp);
   *ld_out = Kp;
   return buf;
+}
+
+template <int E>
+static void launch_nt_nn(const GemmCall& c, bool nn, bool wide, cudaStream_t st) {
+  if (nn) wide ? launch<false, true, 256, false, E>(c, st) : launch<false, true, 128, false, E>(c, st);
+  else wide ? launch<false, false, 256, false, E>(c, st) : launch<false, false, 128, false, E>(c, st);
 }
 
 void gemm_bf16(const GemmCall& c, cudaStream_t st) {
@@ -600,10 +678,22 @@ void gemm_bf16(const GemmCall& c, cudaStream_t st) {
     if (tb) B200_CUDA_CHECK(cudaFreeAsync(tb, st));
     return;
   }
-  switch (c.layout) {
-    case GEMM_NT: wide ? launch<false, false, 256, false>(c, st) : launch<false, false, 128, false>(c, st); break;
-    case GEMM_NN: wide ? launch<false, true, 256, false>(c, st) : launch<false, true, 128, false>(c, st); break;
-    default: wide ? launch<true, true, 256, false>(c, st) : launch<true, true, 128, false>(c, st); break;
+  if (c.layout == GEMM_TN) {
+    wide ? launch<true, true, 256, false>(c, st) : launch<true, true, 128, false>(c, st);
+    return;
+  }
+  // Forward and dgrad GEMMs: a kernel per epilogue the engine runs on them.  With the epilogue chosen at run time,
+  // each of the 16 unrolled column groups carries every epilogue behind branches, and that code costs more than the
+  // main loop; a kernel with one epilogue runs it as straight-line code.
+  const bool nn = c.layout == GEMM_NN;
+  switch (c.epi) {
+    case EPI_NONE: launch_nt_nn<EPI_NONE>(c, nn, wide, st); break;
+    case EPI_BIAS: launch_nt_nn<EPI_BIAS>(c, nn, wide, st); break;
+    case EPI_BIAS_DROP_RES: launch_nt_nn<EPI_BIAS_DROP_RES>(c, nn, wide, st); break;
+    case EPI_BIAS_GELU_DG: launch_nt_nn<EPI_BIAS_GELU_DG>(c, nn, wide, st); break;
+    case EPI_ADD: launch_nt_nn<EPI_ADD>(c, nn, wide, st); break;
+    case EPI_MUL: launch_nt_nn<EPI_MUL>(c, nn, wide, st); break;
+    default: launch_nt_nn<-1>(c, nn, wide, st); break;
   }
 }
 

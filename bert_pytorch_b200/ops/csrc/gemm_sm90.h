@@ -60,6 +60,9 @@ struct GemmCall {
 };
 
 void gemm_bf16(const GemmCall& c, cudaStream_t st);
+// GEMMs of at most `units` work units record their in-kernel timeline into `buf` ([units][16] int64, nullptr: off).
+// Returns whether the kernels were built with -DB200_GEMM_TIMELINE (otherwise nothing is recorded).
+bool gemm_set_timeline(long long* buf, long long units);
 
 CUtensorMap make_tmap_2d_bf16(const void* ptr, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_inner,
                               uint32_t box_outer);
