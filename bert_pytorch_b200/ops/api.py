@@ -16,8 +16,8 @@ from . import extension
 
 # GEMM enums (csrc/gemm_sm90.h)
 NT, NN, TN = 0, 1, 2
-(EPI_NONE, EPI_BIAS, EPI_BIAS_GELU, EPI_BIAS_DROP_RES, EPI_ADD, EPI_DGELU, EPI_ACCUM_F32, EPI_BIAS_TANH, EPI_F32,
- EPI_BIAS_GELU_DG, EPI_MUL) = range(11)
+EPI_NONE, EPI_BIAS, EPI_BIAS_DROP_RES, EPI_ADD, EPI_ACCUM_F32, EPI_BIAS_TANH, EPI_F32, EPI_BIAS_GELU_DG, EPI_MUL = (
+    0, 1, 3, 4, 6, 7, 8, 9, 10)
 
 NUM_SMS = 132           # H100 SXM; only the tile heuristics below use it (the kernels ask the device)
 KERNEL_LAUNCHES = 0     # every wrapper bumps this: bench.py reports it as ``gpu_launches``
@@ -34,10 +34,10 @@ def _count(n: int = 1) -> None:
     KERNEL_LAUNCHES += n
 
 
-# epilogues that read or write a second [M, N] tensor (residual, GELU input or output, keep bits): on 128 x 128 tiles
+# epilogues that read or write a second [M, N] tensor (residual, GELU' or saved factor, keep bits): on 128 x 128 tiles
 # the kernel runs them ping-pong, under the other warpgroup's MMAs, which measured 5-15 % faster on H100 at the
 # BERT-large shapes than the 128 x 256 tile whose two warpgroups run the epilogue together (tools/gemm_bench.py --epi)
-_HEAVY_EPI = (EPI_BIAS_GELU, EPI_BIAS_DROP_RES, EPI_ADD, EPI_DGELU, EPI_BIAS_GELU_DG, EPI_MUL)
+_HEAVY_EPI = (EPI_BIAS_DROP_RES, EPI_ADD, EPI_BIAS_GELU_DG, EPI_MUL)
 
 
 def _pick_block_n(M: int, N: int, epi: int = EPI_NONE) -> int:

@@ -93,6 +93,9 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
     check_bf16(b, "b");
   }
   TORCH_CHECK(a.dim() == 2 && b.dim() == 2 && out.dim() == 2, "gemm operands must be 2-D");
+  TORCH_CHECK(layout == b200::GEMM_NT || layout == b200::GEMM_NN || layout == b200::GEMM_TN, "unknown GEMM layout ", layout);
+  const b200::EpilogueSpec spec = b200::epilogue_spec((int)epi);
+  TORCH_CHECK(spec.name != nullptr, "unknown GEMM epilogue ", epi);
   c10::cuda::CUDAGuard guard(a.device());
   b200::GemmCall c;
   c.layout = (int)layout;
@@ -105,10 +108,9 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
   TORCH_CHECK(out.size(0) == M && out.size(1) == N, "output shape mismatch");
   TORCH_CHECK(a.stride(0) % 8 == 0 && b.stride(0) % 8 == 0, "row strides must be multiples of 8 elements");
   TORCH_CHECK(N % 8 == 0, "N must be a multiple of 8");
-  const bool f32_out = (epi == b200::EPI_ACCUM_F32 || epi == b200::EPI_F32);
   TORCH_CHECK(out.is_cuda() && out.stride(1) == 1, "out must be CUDA with unit inner stride");
-  TORCH_CHECK(out.scalar_type() == (f32_out ? at::kFloat : at::kBFloat16), "out dtype does not match the epilogue");
-  TORCH_CHECK(reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0 && out.stride(0) % (f32_out ? 4 : 8) == 0,
+  TORCH_CHECK(out.scalar_type() == (spec.f32_out ? at::kFloat : at::kBFloat16), "out dtype does not match the epilogue");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0 && out.stride(0) % (spec.f32_out ? 4 : 8) == 0,
               "out must be 16-byte aligned with an aligned row stride");
   c.M = (int)M; c.N = (int)N; c.K = (int)K;
   if (fp8) {
@@ -133,28 +135,23 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
     TORCH_CHECK(res->size(0) == M && res->size(1) == N && res->stride(0) % 8 == 0, "res shape");
     c.res = res->data_ptr(); c.ldr = (int)res->stride(0);
   }
-  const bool needs_bias = epi == b200::EPI_BIAS || epi == b200::EPI_BIAS_GELU || epi == b200::EPI_BIAS_DROP_RES ||
-                          epi == b200::EPI_BIAS_TANH || epi == b200::EPI_BIAS_GELU_DG;
-  TORCH_CHECK(!needs_bias || c.bias != nullptr, "this epilogue needs a bias");
-  TORCH_CHECK((epi != b200::EPI_BIAS_GELU && epi != b200::EPI_BIAS_GELU_DG) || c.aux_out != nullptr, "bias+gelu needs aux_out");
-  TORCH_CHECK(epi != b200::EPI_DGELU || c.res != nullptr, "dgelu needs res (the pre-activation)");
-  TORCH_CHECK(epi != b200::EPI_MUL || c.res != nullptr, "mul needs res");
+  TORCH_CHECK(!spec.bias || c.bias != nullptr, spec.name, " needs a bias");
+  TORCH_CHECK(!spec.aux || c.aux_out != nullptr, spec.name, " needs aux_out");
+  TORCH_CHECK(!spec.res || c.res != nullptr, spec.name, " needs res");
   if (colsum.has_value() && colsum->defined()) {
-    TORCH_CHECK(epi == b200::EPI_NONE || epi == b200::EPI_ADD || epi == b200::EPI_MUL,
-                "column sums are fused into the plain / add / mul epilogues only");
+    TORCH_CHECK(spec.colsum, "column sums are not fused into ", spec.name);
     TORCH_CHECK(colsum->numel() == N && colsum->is_contiguous(), "colsum length");
     c.colsum = opt_f32(colsum);
   }
-  TORCH_CHECK(epi != b200::EPI_BIAS_DROP_RES || c.res != nullptr, "bias+dropout+residual needs res");
   if (mask_out.has_value() && mask_out->defined()) {
-    TORCH_CHECK(epi == b200::EPI_BIAS_DROP_RES && !p_drop_is_zero(p_drop), "mask_out: dropout epilogue only");
+    TORCH_CHECK(spec.keep_bits && !p_drop_is_zero(p_drop), "mask_out: dropout epilogue only");
     TORCH_CHECK(mask_out->is_cuda() && mask_out->scalar_type() == at::kByte && mask_out->is_contiguous() &&
                 mask_out->numel() == M * (N / 8) && reinterpret_cast<uintptr_t>(mask_out->data_ptr()) % 16 == 0 && N % 128 == 0,
                 "mask_out: uint8 [M, N / 8], 16-byte aligned, N % 128 == 0");
     c.mask_out = mask_out->data_ptr<uint8_t>();
   }
   if (mask_in.has_value() && mask_in->defined()) {
-    TORCH_CHECK(epi == b200::EPI_BIAS_DROP_RES && !p_drop_is_zero(p_drop), "mask_in: dropout epilogue only");
+    TORCH_CHECK(spec.keep_bits && !p_drop_is_zero(p_drop), "mask_in: dropout epilogue only");
     TORCH_CHECK(mask_in->is_cuda() && mask_in->scalar_type() == at::kByte && mask_in->is_contiguous() &&
                 mask_in->numel() == M * (N / 8) && reinterpret_cast<uintptr_t>(mask_in->data_ptr()) % 16 == 0 && N % 128 == 0,
                 "mask_in: uint8 [M, N / 8], 16-byte aligned, N % 128 == 0");
@@ -176,7 +173,9 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
     }
   }
   c.stream = (unsigned int)stream_id;
-  b200::gemm_bf16(c, cur_stream());
+  static const char* const form[] = {"NT bf16", "NN bf16", "TN bf16"};
+  TORCH_CHECK(b200::gemm_bf16(c, cur_stream()), "gemm: no kernel is built for ", fp8 ? "fp8" : form[layout],
+              " operands with ", spec.name);
 }
 
 // In-kernel GEMM timeline (tools/gemm_timeline.py): `buf` is int64 [units, 16]; None turns recording off.

@@ -21,11 +21,11 @@
 // fp8 wgmma reads K-major operands only: an MN-major fp8 operand is transposed once into a stream-ordered scratch
 // buffer (fp8_transpose_kernel) and the GEMM runs in the NT form.
 //
-// Epilogues (runtime switch, warp uniform): bias, bias+GELU(erf) with the pre-activation or the derivative saved for
-// backward, bias+dropout+residual, residual add, multiply by GELU'(aux) or by a saved factor, fp32 accumulate-into
-// (wgrad into the gradient arena), bias+tanh, plain fp32.  The accumulator fragment is regrouped inside each quad
-// (quad_transpose) so that a thread owns 8 consecutive output columns: one 16-byte store, one Philox draw and one
-// keep-bit byte per group.
+// Epilogues (a template argument: every kernel carries the straight-line code of one epilogue): bias, bias+GELU(erf)
+// with the derivative saved for backward, bias+dropout+residual, residual add, multiply by a saved factor, fp32
+// accumulate-into (wgrad into the gradient arena), bias+tanh, plain fp32.  gemm_bf16 lists the (operand form,
+// epilogue) pairs that are built.  The accumulator fragment is regrouped inside each quad (quad_transpose) so that a
+// thread owns 8 consecutive output columns: one 16-byte store, one Philox draw and one keep-bit byte per group.
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
@@ -55,7 +55,6 @@ struct GemmArgs {
   int M, N, K;
   int m_blocks, n_blocks, k_blocks, k_splits, k_per_split;
   int units;                 // m_blocks * n_blocks * k_splits
-  int epi;
   void* out;
   int ldo;
   __nv_bfloat16* aux_out;
@@ -104,14 +103,11 @@ struct UnitStamps {
 
 // Epilogue of 8 consecutive output columns [n0, n0 + 8) of one row (n0 % 8 == 0, N % 8 == 0).  `f` holds
 // alpha * accumulator.  Returns through `f` the values that were stored (bf16-rounded) for the column sums.
-// E >= 0: the epilogue is fixed at compile time (must equal p.epi), so a kernel carries the code of that epilogue
-// alone; E < 0: chosen at run time from p.epi.
 template <int E>
 __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8], int row, int n0, unsigned long long seed,
                                                bool add_local) {
-  const int epi = E >= 0 ? E : p.epi;
   const size_t ooff = (size_t)row * p.ldo + n0;
-  if (epi == EPI_ACCUM_F32) {
+  if constexpr (E == EPI_ACCUM_F32) {
     float* o = reinterpret_cast<float*>(p.out) + ooff;
     if (p.peer_world > 1) {
       // an 8-column group crosses at most one shard boundary (shards are multiples of 2048 elements)
@@ -144,29 +140,25 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
                    "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
     return;
   }
-  if (epi == EPI_F32) {
+  if constexpr (E == EPI_F32) {
     float* o = reinterpret_cast<float*>(p.out) + ooff;
     *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
     *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
     return;
   }
-  if (p.bias != nullptr && (epi == EPI_BIAS || epi == EPI_BIAS_GELU || epi == EPI_BIAS_DROP_RES ||
-                            epi == EPI_BIAS_TANH || epi == EPI_BIAS_GELU_DG)) {
-    const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + n0));
-    const uint32_t w[4] = {b.x, b.y, b.z, b.w};
+  if constexpr (epilogue_spec(E).bias) {
+    if (p.bias != nullptr) {
+      const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + n0));
+      const uint32_t w[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const float2 bb = unpack_bf16(w[t]);
-      f[2 * t] += bb.x;
-      f[2 * t + 1] += bb.y;
+      for (int t = 0; t < 4; ++t) {
+        const float2 bb = unpack_bf16(w[t]);
+        f[2 * t] += bb.x;
+        f[2 * t + 1] += bb.y;
+      }
     }
   }
-  if (epi == EPI_BIAS_GELU) {                  // save the pre-activation, then activate
-    *reinterpret_cast<uint4*>(p.aux_out + ooff) =
-        make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-#pragma unroll
-    for (int j = 0; j < 8; ++j) f[j] = gelu_erf(f[j]);
-  } else if (epi == EPI_BIAS_GELU_DG) {
+  if constexpr (E == EPI_BIAS_GELU_DG) {
     float dg[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -176,25 +168,27 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
     }
     *reinterpret_cast<uint4*>(p.aux_out + ooff) =
         make_uint4(pack_bf16(dg[0], dg[1]), pack_bf16(dg[2], dg[3]), pack_bf16(dg[4], dg[5]), pack_bf16(dg[6], dg[7]));
-  } else if (epi == EPI_BIAS_TANH) {
+  } else if constexpr (E == EPI_BIAS_TANH) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) f[j] = tanhf(f[j]);
-  } else if (epi == EPI_BIAS_DROP_RES || epi == EPI_ADD || epi == EPI_DGELU || epi == EPI_MUL) {
-    if (epi == EPI_BIAS_DROP_RES && p.drop_thresh16 != 0) {
-      const size_t moff = (size_t)row * (size_t)(p.N >> 3) + (size_t)(n0 >> 3);
-      uint32_t kb;
-      if (p.mask_in != nullptr) {
-        kb = __ldg(p.mask_in + moff);
-      } else {
-        const uint64_t e8 = ((uint64_t)row * (uint64_t)p.N + (uint64_t)n0) >> 3;
-        const Keep8 keep = dropout_keep8(seed, p.stream, e8, p.drop_thresh16);
-        kb = 0;
+  } else if constexpr (E == EPI_BIAS_DROP_RES || E == EPI_ADD || E == EPI_MUL) {
+    if constexpr (epilogue_spec(E).keep_bits) {
+      if (p.drop_thresh16 != 0) {
+        const size_t moff = (size_t)row * (size_t)(p.N >> 3) + (size_t)(n0 >> 3);
+        uint32_t kb;
+        if (p.mask_in != nullptr) {
+          kb = __ldg(p.mask_in + moff);
+        } else {
+          const uint64_t e8 = ((uint64_t)row * (uint64_t)p.N + (uint64_t)n0) >> 3;
+          const Keep8 keep = dropout_keep8(seed, p.stream, e8, p.drop_thresh16);
+          kb = 0;
 #pragma unroll
-        for (int t = 0; t < 8; ++t) kb |= (keep[t] ? 1u : 0u) << t;
-        if (p.mask_out != nullptr) p.mask_out[moff] = (unsigned char)kb;
+          for (int t = 0; t < 8; ++t) kb |= (keep[t] ? 1u : 0u) << t;
+          if (p.mask_out != nullptr) p.mask_out[moff] = (unsigned char)kb;
+        }
+#pragma unroll
+        for (int t = 0; t < 8; ++t) f[t] = (kb >> t) & 1u ? __fmul_rn(f[t], p.drop_scale) : 0.f;
       }
-#pragma unroll
-      for (int t = 0; t < 8; ++t) f[t] = (kb >> t) & 1u ? __fmul_rn(f[t], p.drop_scale) : 0.f;
     }
     if (p.res != nullptr) {
       const uint4 r = *reinterpret_cast<const uint4*>(p.res + (size_t)row * p.ldr + n0);
@@ -202,10 +196,7 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
         const float2 rr = unpack_bf16(w[t]);
-        if (epi == EPI_DGELU) {
-          f[2 * t] *= dgelu_erf(rr.x);
-          f[2 * t + 1] *= dgelu_erf(rr.y);
-        } else if (epi == EPI_MUL) {
+        if constexpr (E == EPI_MUL) {
           f[2 * t] *= rr.x;
           f[2 * t + 1] *= rr.y;
         } else {
@@ -302,8 +293,6 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const int c = lane & 3;
   const int row_base = row64 + warp * 16 + (lane >> 2);
-  const int epi = E >= 0 ? E : p.epi;
-  const bool bf16_out = epi != EPI_ACCUM_F32 && epi != EPI_F32;
 #pragma unroll
   for (int i = 0; i < NCOLS / 32; ++i) {           // unrolled: the accumulator must stay in registers
     const int n0 = col0 + i * 32 + c * 8;                    // after the regrouping this lane owns columns [n0, n0 + 8)
@@ -326,8 +315,8 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
         float f[8];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
-          // __fmul_rn: never contracted with the bias or residual add that follows (the same rounding as when the
-          // epilogue is chosen at run time and a branch separates the two)
+          // __fmul_rn: alpha * acc is rounded to fp32 before the bias or residual add that follows, so that add is
+          // never contracted into an fma.  The outputs are defined with that rounding.
           f[2 * k] = __fmul_rn(__uint_as_float(lo[k]), alpha);
           f[2 * k + 1] = __fmul_rn(__uint_as_float(hi[k]), alpha);
         }
@@ -336,16 +325,18 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
         for (int t = 0; t < 8; ++t) cs[t] += f[t];
       }
     }
-    if (p.colsum != nullptr && bf16_out) {       // bias gradients: rows of this warp, then one atomic per column
+    if constexpr (!epilogue_spec(E).f32_out) {
+      if (p.colsum != nullptr) {                 // bias gradients: rows of this warp, then one atomic per column
 #pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        cs[t] += __shfl_xor_sync(0xffffffffu, cs[t], 4);
-        cs[t] += __shfl_xor_sync(0xffffffffu, cs[t], 8);
-        cs[t] += __shfl_xor_sync(0xffffffffu, cs[t], 16);
-      }
-      if (lane < 4 && n0 < p.N) {
+        for (int t = 0; t < 8; ++t) {
+          cs[t] += __shfl_xor_sync(0xffffffffu, cs[t], 4);
+          cs[t] += __shfl_xor_sync(0xffffffffu, cs[t], 8);
+          cs[t] += __shfl_xor_sync(0xffffffffu, cs[t], 16);
+        }
+        if (lane < 4 && n0 < p.N) {
 #pragma unroll
-        for (int t = 0; t < 8; ++t) atomicAdd(p.colsum + n0 + t, cs[t]);
+          for (int t = 0; t < 8; ++t) atomicAdd(p.colsum + n0 + t, cs[t]);
+        }
       }
     }
   }
@@ -394,7 +385,7 @@ __device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint6
   }
 }
 
-// E: the epilogue, fixed at compile time (>= 0) or read from p.epi (< 0), see epilogue_group
+// E: the epilogue (GemmEpilogue), see epilogue_group
 template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int E>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -588,7 +579,7 @@ bool gemm_set_timeline(long long* buf, long long units) {
 #endif
 }
 
-template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int E = -1>
+template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int E>
 static void launch(const GemmCall& c, cudaStream_t st) {
   using C = Cfg<BLOCK_N>;
   constexpr int BK = FP8 ? 128 : 64;
@@ -598,7 +589,7 @@ static void launch(const GemmCall& c, cudaStream_t st) {
   p.n_blocks = (c.N + BLOCK_N - 1) / BLOCK_N;
   p.k_blocks = (c.K + BK - 1) / BK;
   if (p.m_blocks <= 0 || p.n_blocks <= 0 || p.k_blocks <= 0) return;
-  int splits = c.epi == EPI_ACCUM_F32 ? c.k_splits : 1;       // only the reducing epilogue can merge K ranges
+  int splits = E == EPI_ACCUM_F32 ? c.k_splits : 1;           // only the reducing epilogue can merge K ranges
   if (splits < 0) {                                            // automatic: fill the machine, >= 4 k-blocks per CTA
     splits = num_sms() / (p.m_blocks * p.n_blocks);
     if (splits > p.k_blocks / 4) splits = p.k_blocks / 4;
@@ -607,7 +598,6 @@ static void launch(const GemmCall& c, cudaStream_t st) {
   if (p.k_splits > p.k_blocks) p.k_splits = p.k_blocks;
   p.k_per_split = (p.k_blocks + p.k_splits - 1) / p.k_splits;
   p.k_splits = (p.k_blocks + p.k_per_split - 1) / p.k_per_split;   // no empty splits
-  p.epi = c.epi;
   p.out = c.out; p.ldo = c.ldo; p.aux_out = reinterpret_cast<__nv_bfloat16*>(c.aux_out);
   p.bias = reinterpret_cast<const __nv_bfloat16*>(c.bias);
   p.res = reinterpret_cast<const __nv_bfloat16*>(c.res); p.ldr = c.ldr;
@@ -651,50 +641,72 @@ static const void* fp8_k_major(const void* src, int mn, int K, int ld, int* ld_o
   return buf;
 }
 
-template <int E>
-static void launch_nt_nn(const GemmCall& c, bool nn, bool wide, cudaStream_t st) {
-  if (nn) wide ? launch<false, true, 256, false, E>(c, st) : launch<false, true, 128, false, E>(c, st);
-  else wide ? launch<false, false, 256, false, E>(c, st) : launch<false, false, 128, false, E>(c, st);
+typedef void (*LaunchFn)(const GemmCall&, cudaStream_t);
+
+// 128 x 256 tiles (wide) or 128 x 128
+template <bool A_MN, bool B_MN, bool FP8, int E>
+static LaunchFn tile_width(bool wide) {
+  return wide ? launch<A_MN, B_MN, 256, FP8, E> : launch<A_MN, B_MN, 128, FP8, E>;
 }
 
-void gemm_bf16(const GemmCall& c, cudaStream_t st) {
+// Operand forms: GEMM_NT, GEMM_NN and GEMM_TN with bf16 operands, and FORM_FP8: fp8 operands in any layout, which run
+// in the NT form once their MN-major operands are transposed.
+constexpr int FORM_FP8 = 3;
+constexpr int form_epi(int form, int epi) { return form * 16 + epi; }
+
+// Every (operand form, epilogue) pair that is built: the pairs the engine, the K-FAC factors, the pretraining and
+// fine-tuning heads, tools/ and the tests call.  nullptr for any other pair.
+static LaunchFn kernel_for(int form, int epi, bool wide) {
+  constexpr bool K_MAJOR = false, MN_MAJOR = true;
+  switch (form_epi(form, epi)) {
+    case form_epi(GEMM_NT, EPI_NONE): return tile_width<K_MAJOR, K_MAJOR, false, EPI_NONE>(wide);
+    case form_epi(GEMM_NT, EPI_BIAS): return tile_width<K_MAJOR, K_MAJOR, false, EPI_BIAS>(wide);
+    case form_epi(GEMM_NT, EPI_BIAS_DROP_RES): return tile_width<K_MAJOR, K_MAJOR, false, EPI_BIAS_DROP_RES>(wide);
+    case form_epi(GEMM_NT, EPI_ADD): return tile_width<K_MAJOR, K_MAJOR, false, EPI_ADD>(wide);
+    case form_epi(GEMM_NT, EPI_MUL): return tile_width<K_MAJOR, K_MAJOR, false, EPI_MUL>(wide);
+    case form_epi(GEMM_NT, EPI_BIAS_GELU_DG): return tile_width<K_MAJOR, K_MAJOR, false, EPI_BIAS_GELU_DG>(wide);
+    case form_epi(GEMM_NT, EPI_BIAS_TANH): return tile_width<K_MAJOR, K_MAJOR, false, EPI_BIAS_TANH>(wide);
+    case form_epi(GEMM_NT, EPI_F32): return tile_width<K_MAJOR, K_MAJOR, false, EPI_F32>(wide);
+    case form_epi(GEMM_NN, EPI_NONE): return tile_width<K_MAJOR, MN_MAJOR, false, EPI_NONE>(wide);
+    case form_epi(GEMM_NN, EPI_ADD): return tile_width<K_MAJOR, MN_MAJOR, false, EPI_ADD>(wide);
+    case form_epi(GEMM_NN, EPI_MUL): return tile_width<K_MAJOR, MN_MAJOR, false, EPI_MUL>(wide);
+    case form_epi(GEMM_TN, EPI_ACCUM_F32): return tile_width<MN_MAJOR, MN_MAJOR, false, EPI_ACCUM_F32>(wide);
+    case form_epi(GEMM_TN, EPI_F32): return tile_width<MN_MAJOR, MN_MAJOR, false, EPI_F32>(wide);
+    case form_epi(FORM_FP8, EPI_NONE): return tile_width<K_MAJOR, K_MAJOR, true, EPI_NONE>(wide);
+    case form_epi(FORM_FP8, EPI_BIAS): return tile_width<K_MAJOR, K_MAJOR, true, EPI_BIAS>(wide);
+    case form_epi(FORM_FP8, EPI_BIAS_DROP_RES): return tile_width<K_MAJOR, K_MAJOR, true, EPI_BIAS_DROP_RES>(wide);
+    case form_epi(FORM_FP8, EPI_ADD): return tile_width<K_MAJOR, K_MAJOR, true, EPI_ADD>(wide);
+    case form_epi(FORM_FP8, EPI_ACCUM_F32): return tile_width<K_MAJOR, K_MAJOR, true, EPI_ACCUM_F32>(wide);
+    case form_epi(FORM_FP8, EPI_F32): return tile_width<K_MAJOR, K_MAJOR, true, EPI_F32>(wide);
+    default: return nullptr;
+  }
+}
+
+bool gemm_bf16(const GemmCall& c, cudaStream_t st) {
   if (c.layout != GEMM_NT && c.layout != GEMM_NN && c.layout != GEMM_TN) {
     fprintf(stderr, "[b200] bad gemm layout %d\n", c.layout);
     abort();
   }
   const bool wide = c.block_n != 128 && c.N > 128;             // 128 x 256 tiles unless the caller asks for 128 x 128
-  if (c.fp8) {
-    if (c.scale_a == nullptr || c.scale_b == nullptr) {
-      fprintf(stderr, "[b200] fp8 gemm needs the device dequantisation factors of both operands\n");
-      abort();
-    }
-    GemmCall k = c;
-    k.layout = GEMM_NT;
-    void* ta = nullptr; void* tb = nullptr;
-    if (c.layout == GEMM_TN) k.A = ta = const_cast<void*>(fp8_k_major(c.A, c.M, c.K, c.lda, &k.lda, st));
-    if (c.layout != GEMM_NT) k.B = tb = const_cast<void*>(fp8_k_major(c.B, c.N, c.K, c.ldb, &k.ldb, st));
-    wide ? launch<false, false, 256, true>(k, st) : launch<false, false, 128, true>(k, st);
-    if (ta) B200_CUDA_CHECK(cudaFreeAsync(ta, st));
-    if (tb) B200_CUDA_CHECK(cudaFreeAsync(tb, st));
-    return;
+  const LaunchFn run = kernel_for(c.fp8 ? FORM_FP8 : c.layout, c.epi, wide);
+  if (run == nullptr) return false;
+  if (!c.fp8) {
+    run(c, st);
+    return true;
   }
-  if (c.layout == GEMM_TN) {
-    wide ? launch<true, true, 256, false>(c, st) : launch<true, true, 128, false>(c, st);
-    return;
+  if (c.scale_a == nullptr || c.scale_b == nullptr) {
+    fprintf(stderr, "[b200] fp8 gemm needs the device dequantisation factors of both operands\n");
+    abort();
   }
-  // Forward and dgrad GEMMs: a kernel per epilogue the engine runs on them.  With the epilogue chosen at run time,
-  // each of the 16 unrolled column groups carries every epilogue behind branches, and that code costs more than the
-  // main loop; a kernel with one epilogue runs it as straight-line code.
-  const bool nn = c.layout == GEMM_NN;
-  switch (c.epi) {
-    case EPI_NONE: launch_nt_nn<EPI_NONE>(c, nn, wide, st); break;
-    case EPI_BIAS: launch_nt_nn<EPI_BIAS>(c, nn, wide, st); break;
-    case EPI_BIAS_DROP_RES: launch_nt_nn<EPI_BIAS_DROP_RES>(c, nn, wide, st); break;
-    case EPI_BIAS_GELU_DG: launch_nt_nn<EPI_BIAS_GELU_DG>(c, nn, wide, st); break;
-    case EPI_ADD: launch_nt_nn<EPI_ADD>(c, nn, wide, st); break;
-    case EPI_MUL: launch_nt_nn<EPI_MUL>(c, nn, wide, st); break;
-    default: launch_nt_nn<-1>(c, nn, wide, st); break;
-  }
+  GemmCall k = c;
+  k.layout = GEMM_NT;
+  void* ta = nullptr; void* tb = nullptr;
+  if (c.layout == GEMM_TN) k.A = ta = const_cast<void*>(fp8_k_major(c.A, c.M, c.K, c.lda, &k.lda, st));
+  if (c.layout != GEMM_NT) k.B = tb = const_cast<void*>(fp8_k_major(c.B, c.N, c.K, c.ldb, &k.ldb, st));
+  run(k, st);
+  if (ta) B200_CUDA_CHECK(cudaFreeAsync(ta, st));
+  if (tb) B200_CUDA_CHECK(cudaFreeAsync(tb, st));
+  return true;
 }
 
 }  // namespace b200

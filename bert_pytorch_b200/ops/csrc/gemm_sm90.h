@@ -12,13 +12,12 @@ enum GemmLayout : int {
   GEMM_TN = 2,  // D[M,N] = A[K,M]^T * B[K,N]        A stored [K][lda], B stored [K][ldb]   (wgrad)
 };
 
+// The values are also those of ops/api.py.
 enum GemmEpilogue : int {
   EPI_NONE = 0,           // out(bf16) = alpha*acc
   EPI_BIAS = 1,           // + bias[n]
-  EPI_BIAS_GELU = 2,      // aux_out = acc + bias ; out = gelu(aux_out)
   EPI_BIAS_DROP_RES = 3,  // out = res + dropout(acc + bias)
   EPI_ADD = 4,            // out = acc + res          (res may be null)
-  EPI_DGELU = 5,          // out = acc * gelu'(res)
   EPI_ACCUM_F32 = 6,      // out(fp32) += alpha*acc   (atomic when split-K)
   EPI_BIAS_TANH = 7,      // out = tanh(acc + bias)
   EPI_F32 = 8,            // out(fp32) = alpha*acc
@@ -26,6 +25,34 @@ enum GemmEpilogue : int {
                           // derivative leave the GEMM together, the backward pass only multiplies -- K16)
   EPI_MUL = 10,           // out = acc * res          (FFN-2 dgrad: res = gelu'(x) saved by EPI_BIAS_GELU_DG)
 };
+
+// What an epilogue reads and writes besides A, B and out.  The binding checks a call's tensors against it and the
+// kernel's epilogue code is compiled from it.
+struct EpilogueSpec {
+  const char* name;   // nullptr: no such epilogue
+  bool f32_out;       // out is fp32 (else bf16)
+  bool bias;          // needs bias[N]
+  bool res;           // needs res[M, N]
+  bool aux;           // writes aux_out[M, N]
+  bool colsum;        // may take colsum: fp32 column sums of the bf16 output
+  bool keep_bits;     // may take mask_in or mask_out: the dropout keep bits
+};
+
+__host__ __device__ constexpr EpilogueSpec epilogue_spec(int epi) {
+  switch (epi) {
+    //                                             f32_out bias   res    aux    colsum keep_bits
+    case EPI_NONE:          return {"EPI_NONE",          false, false, false, false, true,  false};
+    case EPI_BIAS:          return {"EPI_BIAS",          false, true,  false, false, false, false};
+    case EPI_BIAS_DROP_RES: return {"EPI_BIAS_DROP_RES", false, true,  true,  false, false, true};
+    case EPI_ADD:           return {"EPI_ADD",           false, false, false, false, true,  false};
+    case EPI_ACCUM_F32:     return {"EPI_ACCUM_F32",     true,  false, false, false, false, false};
+    case EPI_BIAS_TANH:     return {"EPI_BIAS_TANH",     false, true,  false, false, false, false};
+    case EPI_F32:           return {"EPI_F32",           true,  false, false, false, false, false};
+    case EPI_BIAS_GELU_DG:  return {"EPI_BIAS_GELU_DG",  false, true,  false, true,  false, false};
+    case EPI_MUL:           return {"EPI_MUL",           false, false, true,  false, true,  false};
+    default:                return {nullptr,             false, false, false, false, false, false};
+  }
+}
 
 struct GemmCall {
   int layout = GEMM_NT;
@@ -59,7 +86,9 @@ struct GemmCall {
   float* peer_base[16] = {};
 };
 
-void gemm_bf16(const GemmCall& c, cudaStream_t st);
+// Launches the GEMM.  Returns false, and launches nothing, when no kernel is built for the call's operand form (NT,
+// NN or TN bf16, or fp8) and epilogue.
+bool gemm_bf16(const GemmCall& c, cudaStream_t st);
 // GEMMs of at most `units` work units record their in-kernel timeline into `buf` ([units][16] int64, nullptr: off).
 // Returns whether the kernels were built with -DB200_GEMM_TIMELINE (otherwise nothing is recorded).
 bool gemm_set_timeline(long long* buf, long long units);

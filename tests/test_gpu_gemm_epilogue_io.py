@@ -1,5 +1,5 @@
-"""GEMM epilogues that read a second [M, N] tensor: residual add, GELU' and saved-factor products, bias + dropout +
-residual with given keep bits.  Checked against fp32 torch references at both tile widths: several units per CTA,
+"""GEMM epilogues that read a second [M, N] tensor: residual add, saved-factor product, bias + dropout + residual
+with given keep bits.  Checked against fp32 torch references at both tile widths: several units per CTA,
 residual and output as column slices of wider tensors, ragged tails, keep bits applied bitwise, bitwise replay
 (twice eagerly and from a CUDA graph), and the fp8 path."""
 import math
@@ -34,15 +34,10 @@ def _keep(K_, mask, m, n):
     return ((mask.unsqueeze(-1) >> torch.arange(8, device="cuda", dtype=torch.uint8)) & 1).reshape(m, n).bool()
 
 
-def _dgelu(x):
-    xd = x.double()
-    return (0.5 * (1.0 + torch.erf(xd / math.sqrt(2.0))) + xd * torch.exp(-0.5 * xd * xd) / math.sqrt(2.0 * math.pi)).float()
-
-
 @pytest.mark.parametrize("bn", [128, 256])
 @pytest.mark.parametrize("N,Kd", [(1024, 1024), (4096, 1024), (1024, 4096)])
-def test_every_input_epilogue_many_units(bn, N, Kd):
-    """EPI_ADD, EPI_MUL (+ colsum), EPI_DGELU (NN) and EPI_BIAS_DROP_RES with mask_in (NT) at M = 12288."""
+def test_input_epilogues_many_units(bn, N, Kd):
+    """EPI_ADD and EPI_MUL + colsum (NN), EPI_BIAS_DROP_RES with mask_in (NT) at M = 12288."""
     K_ = _ops()
     a, res = _rand(M, Kd, scale=0.05), _rand(M, N)
     bnn = _rand(Kd, N, scale=0.05)
@@ -52,7 +47,6 @@ def test_every_input_epilogue_many_units(bn, N, Kd):
     out = K_.gemm(a, bnn, layout=K_.NN, epi=K_.EPI_MUL, res=res, colsum=cs, block_n=bn)
     _check(out, ref * res.float())
     assert torch.allclose(cs, out.float().sum(0), rtol=2e-3, atol=2e-2 * math.sqrt(M))
-    _check(K_.gemm(a, bnn, layout=K_.NN, epi=K_.EPI_DGELU, res=res, block_n=bn), ref * _dgelu(res.float()))
     bnt, bias = _rand(N, Kd, scale=0.05), _rand(N)
     x = a.float() @ bnt.float().t() + bias.float()
     mask = K_.dropout_mask(M, N, 0.1, 5, 2, "cuda")
