@@ -139,9 +139,6 @@ class FusedEncoderEngine:
         # the machine with them (+2.5 % on the phase-1 step at 1 and 2 GPUs).  B200_WGRAD_STREAM=0 / ``wgrad_side =
         # False`` keeps everything on one stream.
         self.wgrad_side = os.environ.get("B200_WGRAD_STREAM", "1") != "0"
-        # GELU / GELU' inside the FFN GEMM epilogues (bf16 operand path); B200_FUSED_GELU=0 restores the two
-        # bandwidth kernels
-        self.fused_gelu = os.environ.get("B200_FUSED_GELU", "1") != "0"
         self._wstream = None
         self._wkeep: list = []
 
@@ -357,8 +354,7 @@ class FusedEncoderEngine:
             ctx_q = q[0].view(M, H) if q else None
         # keep bits of the hidden dropout leave the GEMM epilogue (1 bit per element) so that the LayerNorm backward does
         # not have to run Philox again -- bf16 path only
-        keep_bits = (save and ph > 0 and not self.fp8 and H % 128 == 0
-                     and os.environ.get("B200_DROP_MASK", "1") != "0")
+        keep_bits = save and ph > 0 and not self.fp8 and H % 128 == 0
         # ... and are GENERATED by their own kernel (K.dropout_mask: every warp of the machine on Philox) rather than by
         # the GEMM's epilogue warps while the tensor cores idle
         mask1 = K.dropout_mask(M, H, ph, seed, _stream(l, SITE_ATTN_OUT), x.device) if keep_bits else None
@@ -371,7 +367,7 @@ class FusedEncoderEngine:
         x1, mean1, rstd1, *q = K.layer_norm_fwd(pre1, self.p(pre + "attention.output.LayerNorm.weight"),
                                                 self.p(pre + "attention.output.LayerNorm.bias"), save_stats=save,
                                                 fp8=self._side(f"{l}.x1"))
-        if self.fused_gelu and not self.fp8:
+        if not self.fp8:
             # K16: GELU *and* GELU' leave the FFN-1 GEMM through its epilogue (y1 holds gelu'(x), which is all the
             # backward pass needs: the FFN-2 dgrad epilogue multiplies by it) -- no activation pass over HBM at all
             y1 = torch.empty(M, self.I, dtype=torch.bfloat16, device=x1.device)
@@ -450,7 +446,7 @@ class FusedEncoderEngine:
         if kfac is not None:
             kfac.tap(self.prefix + pre + "output.dense", ls.act, d_y2)
         # ---- FFN-2 / GELU'
-        if self.fused_gelu and not self.fp8:
+        if not self.fp8:
             # dgrad epilogue: d_y1 = (d_y2 W2) * gelu'(x) with the FFN-1 bias gradient (column sums) reduced from the
             # staged tile -- the dGELU pass and its bias-gradient pass are gone
             d_y1 = self._lin_bwd(l, "d_y2", "act", "w2", d_y2, ls.act_op, self.w(pre + "output.dense.weight"),

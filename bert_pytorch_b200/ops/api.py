@@ -159,14 +159,14 @@ def _fp8_side(fp8, like: torch.Tensor):
 
 
 def layer_norm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, *, eps: float = 1e-12,
-                   save_stats: bool = True, p_drop: float = 0.0, seed: int = 0, stream: int = 0, fp8=None):
+                   save_stats: bool = True, fp8=None):
     """``fp8=(meta, site)``: also emit the fp8 copy of y (delayed scaling) -> returns (y, mean, rstd, q)."""
     y = torch.empty_like(x)
     M = x.numel() // x.size(-1)
     mean = torch.empty(M, dtype=torch.float32, device=x.device) if save_stats else None
     rstd = torch.empty(M, dtype=torch.float32, device=x.device) if save_stats else None
     q, rec, e5 = _fp8_side(fp8, x)
-    extension().layer_norm_fwd(x, gamma, beta, y, mean, rstd, eps, p_drop, seed, stream, q, rec, e5)
+    extension().layer_norm_fwd(x, gamma, beta, y, mean, rstd, eps, q, rec, e5)
     _count()
     return (y, mean, rstd) if fp8 is None else (y, mean, rstd, q)
 

@@ -186,17 +186,21 @@ bool gemm_timeline(c10::optional<Tensor> buf) {
   return b200::gemm_set_timeline(reinterpret_cast<long long*>(buf->data_ptr<int64_t>()), buf->size(0));
 }
 
+// the LayerNorm kernels cover H % 8 == 0 up to 2048 (8 columns per lane, at most 8 warps or chunks of 256 per row)
+inline void check_ln_width(int64_t H) {
+  TORCH_CHECK(H > 0 && H % 8 == 0 && H <= 2048, "LayerNorm: hidden size ", H, " is not a multiple of 8 in [8, 2048]");
+}
+
 void layer_norm_fwd(Tensor x,Tensor gamma, Tensor beta, Tensor y, c10::optional<Tensor> mean,
-                    c10::optional<Tensor> rstd, double eps, double p_drop, int64_t seed, int64_t stream_id,
-                    c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2) {
+                    c10::optional<Tensor> rstd, double eps, c10::optional<Tensor> q8, c10::optional<Tensor> meta8,
+                    bool e5m2) {
+  check_ln_width(x.size(-1));
   check_bf16(x, "x"); check_bf16(y, "y");
   TORCH_CHECK(x.is_contiguous() && y.is_contiguous(), "x/y must be contiguous");
   const int H = (int)x.size(-1), M = (int)(x.numel() / H);
-  TORCH_CHECK(H % 8 == 0, "hidden size must be a multiple of 8");
   c10::cuda::CUDAGuard guard(x.device());
   b200::layer_norm_fwd(x.data_ptr(), gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(), opt_f32(mean),
-                       opt_f32(rstd), M, H, (float)eps, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
-                       mk_fp8(q8, meta8, e5m2, x.numel()), cur_stream());
+                       opt_f32(rstd), M, H, (float)eps, mk_fp8(q8, meta8, e5m2, x.numel()), cur_stream());
 }
 
 int64_t ln_bwd_workspace(int64_t M, int64_t H) { return b200::ln_bwd_workspace_floats((int)M, (int)H); }
@@ -205,6 +209,7 @@ void layer_norm_bwd(Tensor dy, Tensor x, Tensor mean, Tensor rstd, Tensor gamma,
                     c10::optional<Tensor> dgamma, c10::optional<Tensor> dbeta, c10::optional<Tensor> dbias,
                     Tensor workspace, double p_drop, int64_t seed, int64_t drop_stream, int64_t in_stream,
                     c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2, c10::optional<Tensor> keep_mask) {
+  check_ln_width(x.size(-1));
   check_bf16(dy, "dy"); check_bf16(x, "x"); check_bf16(dx, "dx");
   const int H = (int)x.size(-1), M = (int)(x.numel() / H);
   TORCH_CHECK(workspace.numel() >= b200::ln_bwd_workspace_floats(M, H), "LN workspace too small");

@@ -84,30 +84,6 @@ __device__ __forceinline__ void row_stats(const float (&x)[CHUNKS][8], int H, in
   rstd = rsqrtf(warp_sum(q) / (float)H + eps);
 }
 
-// ------------------------------------------------------------------------------------------------
-// LayerNorm forward / backward, occupancy-friendly layout: WPR warps share one row, every lane owns ONE
-// 16-byte chunk (8 columns), a block holds two such row groups.  ~70-90 registers per thread instead of
-// 255 -> 4-6x more warps in flight, which is what a pure streaming kernel needs to reach HBM speed
-// (first version, one warp per row with 32 columns per lane: 38 us for a 100 MB backward pass).
-// Row statistics travel through shared memory + a named barrier per row group.
-// ------------------------------------------------------------------------------------------------
-// two sums at once across the WPR warps of a row group: ONE named barrier per row -- the exchange slots are
-// double buffered by row parity (a warp can only overwrite parity p again after the barrier of the row in
-// between, which the slowest reader of parity p has to reach first).
-template <int WPR>
-__device__ __forceinline__ float2 group_sum2(float a, float b, float2* slot, int wi, int group) {
-  a = warp_sum(a);
-  b = warp_sum(b);
-  if (WPR == 1) return make_float2(a, b);
-  if ((threadIdx.x & 31) == 0) slot[wi] = make_float2(a, b);
-  if (group == 0) asm volatile("bar.sync 1, %0;" ::"n"(WPR * 32) : "memory");
-  else asm volatile("bar.sync 2, %0;" ::"n"(WPR * 32) : "memory");
-  float2 t = make_float2(0.f, 0.f);
-#pragma unroll
-  for (int w = 0; w < WPR; ++w) { const float2 v = slot[w]; t.x += v.x; t.y += v.y; }
-  return t;
-}
-
 // 16-byte streaming load (read once: do not keep it in L1)
 __device__ __forceinline__ uint4 ld_stream16(const __nv_bfloat16* p) {
   uint4 u;
@@ -139,290 +115,52 @@ __device__ __forceinline__ void store8(__nv_bfloat16* p, const float (&v)[8]) {
                                             pack_bf16(v[6], v[7]));
 }
 
-template <int WPR>
-__global__ void __launch_bounds__(2 * WPR * 32)
-ln_fwd2_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-               __nv_bfloat16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int M, int H,
-               float eps, Seed seed_in, unsigned int stream, unsigned int thresh16, float drop_scale, const Fp8Out f8) {
-  const unsigned long long seed = seed_in.value();
-  const float qscale = f8.q ? f8.meta[1] : 0.f;
-  float amax = 0.f;
-  __shared__ float2 xchg[2][2][8];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int group = warp / WPR, wi = warp % WPR;
-  const int col = (wi * 32 + lane) * 8;
-  const bool live = col < H;
-  float g[8], b[8];
-#pragma unroll
-  for (int t = 0; t < 8; ++t) { g[t] = live ? gamma[col + t] : 0.f; b[t] = live ? beta[col + t] : 0.f; }
-  const int stride = gridDim.x * 2;
-  int row = blockIdx.x * 2 + group;
-  uint4 nx = make_uint4(0, 0, 0, 0);
-  float nshift = 0.f;
-  if (row < M) {
-    if (live) nx = ld_stream16(x + (size_t)row * H + col);
-    nshift = __bfloat162float(x[(size_t)row * H]);
-  }
-  for (int it = 0; row < M; row += stride, ++it) {
-    float v[8];
-    unpack8(nx, v);
-    const float shift = nshift;           // first element of the row: keeps sum / sum-of-squares well conditioned
-    const int nrow = row + stride;
-    if (nrow < M) {                        // prefetch the next row before this row's barrier
-      if (live) nx = ld_stream16(x + (size_t)nrow * H + col);
-      nshift = __bfloat162float(x[(size_t)nrow * H]);
-    }
-    float s = 0.f, q = 0.f;
-    if (live) {
-#pragma unroll
-      for (int t = 0; t < 8; ++t) { const float d = v[t] - shift; s += d; q += d * d; }
-    }
-    const float2 r = group_sum2<WPR>(s, q, xchg[group][it & 1], wi, group);
-    const float ms = r.x / (float)H;
-    const float mean = shift + ms;
-    const float rstd = rsqrtf(fmaxf(r.y / (float)H - ms * ms, 0.f) + eps);
-    if (live) {
-      Keep8 keep = Keep8::all();
-      if (thresh16 != 0) keep = dropout_keep8(seed, stream, ((uint64_t)row * H + col) >> 3, thresh16);
-#pragma unroll
-      for (int t = 0; t < 8; ++t) {
-        float o = (v[t] - mean) * rstd * g[t] + b[t];
-        if (thresh16 != 0) o = keep[t] ? o * drop_scale : 0.f;
-        v[t] = o;
-      }
-      store8(y + (size_t)row * H + col, v);
-      if (f8.q) fp8_emit8(f8, (size_t)row * H + col, v, qscale, amax);
-    }
-    if (wi == 0 && lane == 0) {
-      if (mean_out) mean_out[row] = mean;
-      if (rstd_out) rstd_out[row] = rstd;
-    }
-  }
-  if (f8.q) fp8_amax_commit(f8, amax);
-}
-
-// Opt-in variant (B200_LN_ROWS=2): every group of WPR warps works on TWO rows per iteration -- twice the bytes in
-// flight per thread (the kernel above is latency bound: 16 B per thread and one barrier per row) and one barrier per
-// two rows.  Same arithmetic per row, so the results are bit-identical to ln_fwd2_kernel.
-template <int WPR>
-__device__ __forceinline__ float4 group_sum4(float a, float b, float c, float d, float4* slot, int wi, int group) {
-  a = warp_sum(a); b = warp_sum(b); c = warp_sum(c); d = warp_sum(d);
-  if (WPR == 1) return make_float4(a, b, c, d);
-  if ((threadIdx.x & 31) == 0) slot[wi] = make_float4(a, b, c, d);
-  if (group == 0) asm volatile("bar.sync 1, %0;" ::"n"(WPR * 32) : "memory");
-  else asm volatile("bar.sync 2, %0;" ::"n"(WPR * 32) : "memory");
-  float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int w = 0; w < WPR; ++w) { const float4 v = slot[w]; t.x += v.x; t.y += v.y; t.z += v.z; t.w += v.w; }
-  return t;
-}
-
-template <int WPR>
-__global__ void __launch_bounds__(2 * WPR * 32)
-ln_fwd2x2_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                 __nv_bfloat16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int M, int H,
-                 float eps, Seed seed_in, unsigned int stream, unsigned int thresh16, float drop_scale, const Fp8Out f8) {
-  const unsigned long long seed = seed_in.value();
-  const float qscale = f8.q ? f8.meta[1] : 0.f;
-  float amax = 0.f;
-  __shared__ float4 xchg[2][2][8];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int group = warp / WPR, wi = warp % WPR;
-  const int col = (wi * 32 + lane) * 8;
-  const bool live = col < H;
-  float g[8], b[8];
-#pragma unroll
-  for (int t = 0; t < 8; ++t) { g[t] = live ? gamma[col + t] : 0.f; b[t] = live ? beta[col + t] : 0.f; }
-  const int stride = gridDim.x * 4;                 // 2 groups x 2 rows per block and iteration
-  int row = (blockIdx.x * 2 + group) * 2;           // this group's rows: row, row + 1
-  uint4 nx[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-  float nshift[2] = {0.f, 0.f};
-#pragma unroll
-  for (int r = 0; r < 2; ++r)
-    if (row + r < M) {
-      if (live) nx[r] = ld_stream16(x + (size_t)(row + r) * H + col);
-      nshift[r] = __bfloat162float(x[(size_t)(row + r) * H]);
-    }
-  for (int it = 0; row < M; row += stride, ++it) {
-    float v[2][8], shift[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) { unpack8(nx[r], v[r]); shift[r] = nshift[r]; }
-    const int nrow = row + stride;
-#pragma unroll
-    for (int r = 0; r < 2; ++r)
-      if (nrow + r < M) {                  // prefetch the next pair before this pair's barrier
-        if (live) nx[r] = ld_stream16(x + (size_t)(nrow + r) * H + col);
-        nshift[r] = __bfloat162float(x[(size_t)(nrow + r) * H]);
-      }
-    float s[2] = {0.f, 0.f}, q[2] = {0.f, 0.f};
-    if (live) {
-#pragma unroll
-      for (int r = 0; r < 2; ++r)
-#pragma unroll
-        for (int t = 0; t < 8; ++t) { const float d = v[r][t] - shift[r]; s[r] += d; q[r] += d * d; }
-    }
-    const float4 red = group_sum4<WPR>(s[0], q[0], s[1], q[1], xchg[group][it & 1], wi, group);
-    const float rs[2] = {red.x, red.z}, rq[2] = {red.y, red.w};
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int rr = row + r;
-      if (rr >= M) continue;
-      const float ms = rs[r] / (float)H;
-      const float mean = shift[r] + ms;
-      const float rstd = rsqrtf(fmaxf(rq[r] / (float)H - ms * ms, 0.f) + eps);
-      if (live) {
-        Keep8 keep = Keep8::all();
-        if (thresh16 != 0) keep = dropout_keep8(seed, stream, ((uint64_t)rr * H + col) >> 3, thresh16);
-#pragma unroll
-        for (int t = 0; t < 8; ++t) {
-          float o = (v[r][t] - mean) * rstd * g[t] + b[t];
-          if (thresh16 != 0) o = keep[t] ? o * drop_scale : 0.f;
-          v[r][t] = o;
-        }
-        store8(y + (size_t)rr * H + col, v[r]);
-        if (f8.q) fp8_emit8(f8, (size_t)rr * H + col, v[r], qscale, amax);
-      }
-      if (wi == 0 && lane == 0) {
-        if (mean_out) mean_out[rr] = mean;
-        if (rstd_out) rstd_out[rr] = rstd;
-      }
-    }
-  }
-  if (f8.q) fp8_amax_commit(f8, amax);
-}
-
-// LayerNorm backward.
-//   in : dy [M,H] (grad wrt LN output; with `in_stream` given, dy is first multiplied by the *output* dropout
-//        mask of that stream -- used by the embedding LN whose output was dropped out)
-//        x  [M,H] pre-LN input, mean/rstd [M], gamma [H]
-//   out: dx [M,H]          grad wrt the pre-LN input (this is also the residual-branch gradient)
-//        dxd [M,H] optional: dx * dropout_mask(stream `drop_stream`) * scale  -> gradient of the GEMM output
-//                            that was dropped out before the residual add (K14/K18)
-//        partial [grid, 3, H]: per-block column sums of (dy*xhat, dy, dxd) -> dgamma, dbeta, dbias
-template <int WPR>
-__global__ void __launch_bounds__(2 * WPR * 32)
-ln_bwd2_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
-               const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ gamma,
-               __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dxd, float* __restrict__ partial, int M,
-               int H, Seed seed_in, unsigned int drop_stream, unsigned int in_stream,
-               unsigned int thresh16, float drop_scale, const Fp8Out f8) {
-  const unsigned long long seed = seed_in.value();
-  const float qscale = f8.q ? f8.meta[1] : 0.f;
-  float amax = 0.f;
-  __shared__ float2 xchg[2][2][8];
-  __shared__ float comb[3][WPR * 256];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int group = warp / WPR, wi = warp % WPR;
-  const int col = (wi * 32 + lane) * 8;
-  const bool live = col < H;
-  float g[8], ag[8], ab[8], ad[8];
-#pragma unroll
-  for (int t = 0; t < 8; ++t) { g[t] = live ? gamma[col + t] : 0.f; ag[t] = ab[t] = ad[t] = 0.f; }
-  const int stride = gridDim.x * 2;
-  int row = blockIdx.x * 2 + group;
-  uint4 nd = make_uint4(0, 0, 0, 0), nv = make_uint4(0, 0, 0, 0);
-  float nmu = 0.f, nrs = 0.f;
-  if (row < M) {
-    if (live) { nd = ld_stream16(dy + (size_t)row * H + col); nv = ld_stream16(x + (size_t)row * H + col); }
-    nmu = mean[row]; nrs = rstd[row];
-  }
-  for (int it = 0; row < M; row += stride, ++it) {
-    float d[8], v[8];
-    unpack8(nd, d);
-    unpack8(nv, v);
-    const float mu = nmu, rs = nrs;
-    const int nrow = row + stride;
-    if (nrow < M) {                        // next row's loads are in flight across this row's barrier
-      if (live) { nd = ld_stream16(dy + (size_t)nrow * H + col); nv = ld_stream16(x + (size_t)nrow * H + col); }
-      nmu = mean[nrow]; nrs = rstd[nrow];
-    }
-    if (in_stream != 0xFFFFFFFFu && thresh16 != 0 && live) {
-      const Keep8 keep = dropout_keep8(seed, in_stream, ((uint64_t)row * H + col) >> 3, thresh16);
-#pragma unroll
-      for (int t = 0; t < 8; ++t) d[t] = keep[t] ? d[t] * drop_scale : 0.f;
-    }
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-      const float xh = live ? (v[t] - mu) * rs : 0.f;
-      const float dg = d[t] * g[t];
-      ag[t] += d[t] * xh;
-      ab[t] += d[t];
-      v[t] = xh;
-      d[t] = dg;
-      s1 += dg;
-      s2 += dg * xh;
-    }
-    const float2 r = group_sum2<WPR>(s1, s2, xchg[group][it & 1], wi, group);
-    s1 = r.x / (float)H;
-    s2 = r.y / (float)H;
-    if (live) {
-#pragma unroll
-      for (int t = 0; t < 8; ++t) d[t] = rs * (d[t] - s1 - v[t] * s2);
-      store8(dx + (size_t)row * H + col, d);
-      if (dxd != nullptr) {
-        if (thresh16 != 0) {
-          const Keep8 keep = dropout_keep8(seed, drop_stream, ((uint64_t)row * H + col) >> 3, thresh16);
-#pragma unroll
-          for (int t = 0; t < 8; ++t) d[t] = keep[t] ? d[t] * drop_scale : 0.f;
-        }
-#pragma unroll
-        for (int t = 0; t < 8; ++t) ad[t] += d[t];
-        store8(dxd + (size_t)row * H + col, d);
-        if (f8.q) fp8_emit8(f8, (size_t)row * H + col, d, qscale, amax);
-      }
-    }
-  }
-  if (f8.q) fp8_amax_commit(f8, amax);
-  // combine the two row groups of the block and write the per-block partial column sums
-  const int cbase = (wi * 32 + lane) * 8;
-  if (group == 1) {
-#pragma unroll
-    for (int t = 0; t < 8; ++t) { comb[0][cbase + t] = ag[t]; comb[1][cbase + t] = ab[t]; comb[2][cbase + t] = ad[t]; }
-  }
-  __syncthreads();
-  if (group == 0 && live) {
-    float* dst = partial + (size_t)blockIdx.x * 3 * H + col;
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-      dst[t] = ag[t] + comb[0][cbase + t];
-      dst[H + t] = ab[t] + comb[1][cbase + t];
-      dst[2 * H + t] = ad[t] + comb[2][cbase + t];
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// Fast paths (H == CHUNKS * 256, no fp8 side output).  The kernels above are instruction bound (per-row reductions,
-// barriers and address arithmetic amortised over only 8 elements per lane), so these variants cut instructions per element:
-//   forward : one warp owns a whole row (32 elements per lane): shuffle-only statistics, exact two-pass variance in
-//             registers, gamma / beta from shared memory (conflict-free float4 layout); ~8 instructions per element
-//   backward: same lane-owns-8-columns layout as ln_bwd2 (the column sums for dgamma / dbeta / dbias must stay in
-//             registers of a fixed lane) but without bounds predicates, with the per-row constants folded into two
-//             FFMAs per element, one 64-bit Philox counter computation per row.
+// LayerNorm forward / backward.  Both are instruction bound at these sizes (per-row reductions and address arithmetic
+// amortised over few elements per lane), so they keep the instructions per element low:
+//   forward : one warp owns a whole row (8 columns per lane and 256-column chunk): shuffle-only statistics, exact
+//             two-pass variance in registers, gamma / beta from shared memory (conflict-free float4 layout)
+//   backward: WPR warps share a row and every lane owns 8 columns (the column sums for dgamma / dbeta / dbias stay in
+//             registers of a fixed lane), the per-row constants are folded into two FFMAs per element, one 64-bit
+//             Philox counter computation per row.
+// TAIL = false: H is CHUNKS * 256 (WPR * 256) at compile time, no bounds predicates.  TAIL = true: H (a multiple of 8)
+// is a kernel argument and the 8-column groups at or past H are predicated off.  FP8: the fp8 copy of the output
+// (Fp8Out) is written in the same pass.
 // ------------------------------------------------------------------------------------------------
-template <int CHUNKS>
+template <int CHUNKS, bool TAIL, bool FP8>
 __global__ void __launch_bounds__(256)
 ln_fwd_row_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
                   __nv_bfloat16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int M,
-                  float eps) {
-  constexpr int H = CHUNKS * 256;
+                  float eps, int h, const Fp8Out f8) {
+  const int H = TAIL ? h : CHUNKS * 256;
   __shared__ float4 sg[CHUNKS][2][32], sb[CHUNKS][2][32];   // [chunk][half of the lane's 8 columns][lane]
   pdl_trigger_small();
   pdl_wait();
   for (int i = threadIdx.x; i < CHUNKS * 64; i += blockDim.x) {
-    const int c = i >> 6, h = (i >> 5) & 1, l = i & 31;
-    sg[c][h][l] = __ldg(reinterpret_cast<const float4*>(gamma + c * 256 + l * 8 + h * 4));
-    sb[c][h][l] = __ldg(reinterpret_cast<const float4*>(beta + c * 256 + l * 8 + h * 4));
+    const int c = i >> 6, hf = (i >> 5) & 1, l = i & 31;
+    const int col = c * 256 + l * 8 + hf * 4;
+    if (!TAIL || col < H) {
+      sg[c][hf][l] = __ldg(reinterpret_cast<const float4*>(gamma + col));
+      sb[c][hf][l] = __ldg(reinterpret_cast<const float4*>(beta + col));
+    }
   }
   __syncthreads();
+  const float qscale = FP8 ? f8.meta[1] : 0.f;
+  float amax = 0.f;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane_cols = H - lane * 8;      // chunk c of this lane lies inside the row iff c * 256 < lane_cols
+  auto live = [&](int c) { return !TAIL || c * 256 < lane_cols; };
   const int stride = gridDim.x * 8;
   int row = blockIdx.x * 8 + warp;
   uint4 nx[CHUNKS];
+  if constexpr (TAIL) {                    // columns past H read as zeros: they add nothing to the row sum
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) nx[c] = make_uint4(0, 0, 0, 0);
+  }
   if (row < M) {
 #pragma unroll
-    for (int c = 0; c < CHUNKS; ++c) nx[c] = ld_stream16(x + (size_t)row * H + c * 256 + lane * 8);
+    for (int c = 0; c < CHUNKS; ++c)
+      if (live(c)) nx[c] = ld_stream16(x + (size_t)row * H + c * 256 + lane * 8);
   }
   for (; row < M; row += stride) {
     float v[CHUNKS][8];
@@ -431,7 +169,8 @@ ln_fwd_row_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__
     const int nrow = row + stride;
     if (nrow < M) {                        // next row in flight while this one is reduced
 #pragma unroll
-      for (int c = 0; c < CHUNKS; ++c) nx[c] = ld_stream16(x + (size_t)nrow * H + c * 256 + lane * 8);
+      for (int c = 0; c < CHUNKS; ++c)
+        if (live(c)) nx[c] = ld_stream16(x + (size_t)nrow * H + c * 256 + lane * 8);
     }
     float s = 0.f;
 #pragma unroll
@@ -442,48 +181,67 @@ ln_fwd_row_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__
     float q = 0.f;
 #pragma unroll
     for (int c = 0; c < CHUNKS; ++c)
+      if (live(c)) {
 #pragma unroll
-      for (int t = 0; t < 8; ++t) { v[c][t] -= mean; q = fmaf(v[c][t], v[c][t], q); }
+        for (int t = 0; t < 8; ++t) { v[c][t] -= mean; q = fmaf(v[c][t], v[c][t], q); }
+      }
     const float rstd = rsqrtf(warp_sum(q) * (1.0f / (float)H) + eps);
 #pragma unroll
     for (int c = 0; c < CHUNKS; ++c) {
+      if (!live(c)) continue;
       const float4 g0 = sg[c][0][lane], g1 = sg[c][1][lane], b0 = sb[c][0][lane], b1 = sb[c][1][lane];
       const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
       const float b[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
       for (int t = 0; t < 8; ++t) v[c][t] = fmaf(v[c][t] * rstd, g[t], b[t]);
       store8(y + (size_t)row * H + c * 256 + lane * 8, v[c]);
+      if constexpr (FP8) fp8_emit8(f8, (size_t)row * H + c * 256 + lane * 8, v[c], qscale, amax);
     }
     if (lane == 0) {
       if (mean_out) mean_out[row] = mean;
       if (rstd_out) rstd_out[row] = rstd;
     }
   }
+  if constexpr (FP8) fp8_amax_commit(f8, amax);
 }
 
-template <int WPR, int GROUPS>
+// LayerNorm backward, GROUPS rows per block at a time.
+//   in : dy [M,H] grad wrt the LN output; with `in_stream` given (TAIL instantiations only), dy is first multiplied by
+//        the output dropout of that stream -- the embedding LN, whose output was dropped out
+//        x [M,H] pre-LN input, mean / rstd [M], gamma [H]
+//   out: dx [M,H]  grad wrt the pre-LN input (also the residual-branch gradient)
+//        dxd [M,H] optional: dx * dropout_mask(stream `drop_stream`) * scale, the gradient of the GEMM output that was
+//                  dropped out before the residual add.  The keep decisions are READ from `keep_mask` (one byte per 8
+//                  elements, written by dropout_mask_kernel or by the producing GEMM epilogue: GemmCall::mask_out)
+//                  instead of regenerated with Philox whenever the caller has them.
+//        partial [grid, 3, H]: per-block column sums of (dy * xhat, dy, dxd) -> dgamma, dbeta, dbias
+template <int WPR, int GROUPS, bool TAIL, bool FP8>
 __global__ void __launch_bounds__(GROUPS * WPR * 32)
 ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
                const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ gamma,
                __nv_bfloat16* __restrict__ dx, __nv_bfloat16* __restrict__ dxd, float* __restrict__ partial, int M,
                Seed seed_in, unsigned int drop_stream, unsigned int thresh16, float drop_scale,
-               const uint8_t* __restrict__ keep_mask) {
-  // The dropout decisions of the residual branch are READ (one byte per 8 elements, written by dropout_mask_kernel
-  // or by the producing GEMM epilogue: GemmCall::mask_out) instead of regenerated with Philox whenever the caller
-  // has them.
-  constexpr int H = WPR * 256;
+               const uint8_t* __restrict__ keep_mask, int h, unsigned int in_stream, const Fp8Out f8) {
+  const int H = TAIL ? h : WPR * 256;
   __shared__ float2 xchg[GROUPS][2][WPR];
-  __shared__ float comb[GROUPS - 1 > 0 ? GROUPS - 1 : 1][3][H];
+  __shared__ float comb[GROUPS - 1 > 0 ? GROUPS - 1 : 1][3][WPR * 256];
   pdl_trigger_small();
   pdl_wait();
   const unsigned long long seed = thresh16 != 0 ? seed_in.value() : 0ull;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int group = warp / WPR, wi = warp % WPR;
   const int col = (wi * 32 + lane) * 8;
+  const bool live = !TAIL || col < H;      // this lane's 8 columns lie inside the row
+  const bool in_drop = TAIL && in_stream != 0xFFFFFFFFu && thresh16 != 0;
+  const float qscale = FP8 ? f8.meta[1] : 0.f;
+  float amax = 0.f;
   f32x2 g2[4], ag2[4], ab2[4], ad2[4];
   {
-    const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + col));
-    const float4 g1 = __ldg(reinterpret_cast<const float4*>(gamma + col + 4));
+    float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
+    if (live) {
+      g0 = __ldg(reinterpret_cast<const float4*>(gamma + col));
+      g1 = __ldg(reinterpret_cast<const float4*>(gamma + col + 4));
+    }
     g2[0] = f2_pack(g0.x, g0.y); g2[1] = f2_pack(g0.z, g0.w); g2[2] = f2_pack(g1.x, g1.y); g2[3] = f2_pack(g1.z, g1.w);
   }
 #pragma unroll
@@ -494,31 +252,38 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
   float nmu = 0.f, nrs = 0.f;
   uint32_t nmask = 0;
   const bool use_mask = keep_mask != nullptr && dxd != nullptr && thresh16 != 0;
-  if (row < M) {
-    nd = ld_stream16(dy + (size_t)row * H + col);
-    nv = ld_stream16(x + (size_t)row * H + col);
+  if (row < M) {                           // columns past H read as zeros: they add nothing to the sums
+    if (live) {
+      nd = ld_stream16(dy + (size_t)row * H + col);
+      nv = ld_stream16(x + (size_t)row * H + col);
+    }
     nmu = __ldg(mean + row);
     nrs = __ldg(rstd + row);
-    if (use_mask) nmask = __ldg(keep_mask + (size_t)row * (H / 8) + (col >> 3));
+    if (use_mask && live) nmask = __ldg(keep_mask + (size_t)row * (H / 8) + (col >> 3));
   }
-  constexpr float invH = 1.0f / (float)H;
+  const float invH = 1.0f / (float)H;
   for (int it = 0; row < M; row += stride, ++it) {
     const uint32_t dw[4] = {nd.x, nd.y, nd.z, nd.w}, vw[4] = {nv.x, nv.y, nv.z, nv.w};
     const float rs = nrs, nmr = -nmu * nrs;
     const uint32_t mask = nmask;
     const int nrow = row + stride;
     if (nrow < M) {                        // next row's loads are in flight across this row's barrier
-      nd = ld_stream16(dy + (size_t)nrow * H + col);
-      nv = ld_stream16(x + (size_t)nrow * H + col);
+      if (live) {
+        nd = ld_stream16(dy + (size_t)nrow * H + col);
+        nv = ld_stream16(x + (size_t)nrow * H + col);
+      }
       nmu = __ldg(mean + nrow);
       nrs = __ldg(rstd + nrow);
-      if (use_mask) nmask = __ldg(keep_mask + (size_t)nrow * (H / 8) + (col >> 3));
+      if (use_mask && live) nmask = __ldg(keep_mask + (size_t)nrow * (H / 8) + (col >> 3));
     }
+    Keep8 in_keep = Keep8::all();
+    if (in_drop) in_keep = dropout_keep8(seed, in_stream, (uint64_t)row * (uint64_t)(H / 8) + (uint64_t)(col >> 3), thresh16);
     const f32x2 rs2 = f2_splat(rs), nmr2 = f2_splat(nmr);
     f32x2 xh[4], dg[4], s1p = f2_splat(0.f), s2p = f2_splat(0.f);
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
-      const f32x2 d = f2_from_bf16x2(dw[t]);
+      f32x2 d = f2_from_bf16x2(dw[t]);
+      if (in_drop) d = f2_mul(d, f2_pack(in_keep[2 * t] ? drop_scale : 0.f, in_keep[2 * t + 1] ? drop_scale : 0.f));
       xh[t] = f2_fma(f2_from_bf16x2(vw[t]), rs2, nmr2);
       dg[t] = f2_mul(d, g2[t]);
       ag2[t] = f2_fma(d, xh[t], ag2[t]);
@@ -542,6 +307,7 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
     f32x2 o[4];
 #pragma unroll
     for (int t = 0; t < 4; ++t) o[t] = f2_fma(xh[t], c2, f2_fma(dg[t], rs2, c1));   // rs (dg - mean(dg) - xh mean(dg xh))
+    if (!live) continue;
     const size_t off = (size_t)row * H + col;
     *reinterpret_cast<uint4*>(dx + off) = make_uint4(f2_to_bf16x2(o[0]), f2_to_bf16x2(o[1]), f2_to_bf16x2(o[2]), f2_to_bf16x2(o[3]));
     if (dxd != nullptr) {
@@ -560,8 +326,15 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
 #pragma unroll
       for (int t = 0; t < 4; ++t) ad2[t] = f2_add(ad2[t], o[t]);
       *reinterpret_cast<uint4*>(dxd + off) = make_uint4(f2_to_bf16x2(o[0]), f2_to_bf16x2(o[1]), f2_to_bf16x2(o[2]), f2_to_bf16x2(o[3]));
+      if constexpr (FP8) {
+        float r[8];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) { r[2 * t] = o[t].x; r[2 * t + 1] = o[t].y; }
+        fp8_emit8(f8, off, r, qscale, amax);
+      }
     }
   }
+  if constexpr (FP8) fp8_amax_commit(f8, amax);
   float ag[8], ab[8], ad[8];
 #pragma unroll
   for (int t = 0; t < 4; ++t) {
@@ -590,7 +363,7 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
         }
     }
   }
-  if (group == 0) {           // per-block partial column sums; colsum_finalize_kernel adds them into the gradient arena
+  if (group == 0 && live) {   // per-block partial column sums; colsum_finalize_kernel adds them into the gradient arena
     // (444 blocks x 3072 same-address atomics at the end of the kernel serialise in L2: measured 2x slower)
     float* dst = partial + (size_t)blockIdx.x * 3 * H + col;
     *reinterpret_cast<float4*>(dst) = make_float4(ag[0], ag[1], ag[2], ag[3]);
@@ -604,9 +377,9 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
 
 // dst[k][col] += sum over blocks of partial[block][k][col]   (k = 0..2, any dst may be null)
 // grid (ceil(H/32), 3, Z), 256 threads: warp w sums rows w, w+8, ... of a 32-column strip (coalesced 128 B
-// per row), then the 8 warps are combined through shared memory.  Z > 1 (B200_LN_FINALIZE_SPLIT, opt-in) cuts the
-// partial rows into Z slices that finish with an atomic add: the kernel is a chain of ~55 dependent loads per warp
-// at Z = 1 (8 us for 444 partial rows), i.e. latency bound.
+// per row), then the 8 warps are combined through shared memory.  Z > 1 cuts the partial rows into Z slices that
+// finish with an atomic add: the kernel is a chain of ~55 dependent loads per warp at Z = 1 (8 us for 444 partial
+// rows), i.e. latency bound.
 __global__ void __launch_bounds__(256)
 colsum_finalize_kernel(const float* __restrict__ partial, int nblocks, int H, float* dgamma, float* dbeta,
                        float* dbias) {
@@ -971,64 +744,34 @@ static inline int ln_grid(int M) {
     else { fprintf(stderr, "[b200] hidden size %d too large for the LN kernels\n", (H)); abort(); } \
   } while (0)
 
-#define DISPATCH_WPR(H, ...)                                         \
-  do {                                                               \
-    const int wpr_ = ((H) + 255) / 256;                              \
-    if (wpr_ <= 1) { constexpr int WPR = 1; __VA_ARGS__; }           \
-    else if (wpr_ <= 2) { constexpr int WPR = 2; __VA_ARGS__; }      \
-    else if (wpr_ <= 3) { constexpr int WPR = 3; __VA_ARGS__; }      \
-    else if (wpr_ <= 4) { constexpr int WPR = 4; __VA_ARGS__; }      \
-    else if (wpr_ <= 8) { constexpr int WPR = 8; __VA_ARGS__; }      \
-    else { fprintf(stderr, "[b200] hidden size %d too large for the LN kernels\n", (H)); abort(); } \
-  } while (0)
-
-static inline int ln2_grid(int M) {     // 2 rows per block at a time; 4 resident blocks per SM
-  int g = (M + 1) / 2;
-  return g < num_sms() * 4 ? g : num_sms() * 4;
-}
-
-static bool ln_fast_enabled() {
-  static const bool on = []() { const char* e = getenv("B200_LN_FAST"); return !(e && e[0] == '0'); }();
-  return on;
-}
-
 void layer_norm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int M,
-                    int H, float eps, Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st) {
-  unsigned int th; float sc;
-  drop_params(p_drop, th, sc);
-  if (ln_fast_enabled() && th == 0 && f8.q == nullptr && H % 256 == 0 && H <= 1024) {   // warp-per-row fast path
-    int g = (M + 7) / 8;
-    if (g > num_sms() * 4) g = num_sms() * 4;
-    const __nv_bfloat16* xp = (const __nv_bfloat16*)x;
-    __nv_bfloat16* yp = (__nv_bfloat16*)y;
-    switch (H / 256) {
-      case 1: launch_pdl(ln_fwd_row_kernel<1>, dim3(g), dim3(256), 0, st, xp, gamma, beta, yp, mean, rstd, M, eps); break;
-      case 2: launch_pdl(ln_fwd_row_kernel<2>, dim3(g), dim3(256), 0, st, xp, gamma, beta, yp, mean, rstd, M, eps); break;
-      case 3: launch_pdl(ln_fwd_row_kernel<3>, dim3(g), dim3(256), 0, st, xp, gamma, beta, yp, mean, rstd, M, eps); break;
-      default: launch_pdl(ln_fwd_row_kernel<4>, dim3(g), dim3(256), 0, st, xp, gamma, beta, yp, mean, rstd, M, eps); break;
-    }
-    return;
-  }
-  static const bool two_rows = []() { const char* e = getenv("B200_LN_ROWS"); return e && e[0] == '2'; }();
-  if (two_rows) {                        // measured slower than one row (24.6 vs 22.6 us): kept for reference only
-    int g4 = (M + 3) / 4;
-    if (g4 > num_sms() * 3) g4 = num_sms() * 3;
-    DISPATCH_WPR(H, (ln_fwd2x2_kernel<WPR><<<g4, 2 * WPR * 32, 0, st>>>(
-        (const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, M, H, eps, seed, stream, th, sc, f8)));
-    return;
-  }
-  DISPATCH_WPR(H, (ln_fwd2_kernel<WPR><<<ln2_grid(M), 2 * WPR * 32, 0, st>>>(
-      (const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, M, H, eps, seed, stream, th, sc, f8)));
+                    int H, float eps, Fp8Out f8, cudaStream_t st) {
+  decltype(&ln_fwd_row_kernel<1, false, false>) k;
+  if (f8.q == nullptr && H % 256 == 0 && H <= 1024)      // the encoder LNs of the bf16 path
+    k = H == 256 ? ln_fwd_row_kernel<1, false, false> : H == 512 ? ln_fwd_row_kernel<2, false, false>
+      : H == 768 ? ln_fwd_row_kernel<3, false, false> : ln_fwd_row_kernel<4, false, false>;
+  else if (f8.q == nullptr)
+    k = H <= 512 ? ln_fwd_row_kernel<2, true, false> : H <= 1024 ? ln_fwd_row_kernel<4, true, false>
+                                                                 : ln_fwd_row_kernel<8, true, false>;
+  else
+    k = H <= 512 ? ln_fwd_row_kernel<2, true, true> : H <= 1024 ? ln_fwd_row_kernel<4, true, true>
+                                                                : ln_fwd_row_kernel<8, true, true>;
+  int g = (M + 7) / 8;
+  if (g > num_sms() * 4) g = num_sms() * 4;
+  launch_pdl(k, dim3(g), dim3(256), 0, st, (const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, M, eps,
+             H, f8);
 }
 
-// backward: ~80 registers x 256 threads -> 3 blocks per SM are co-resident; one exact wave (a grid of 4 per SM
-// ran a 1/3-full second wave)
-static inline int ln2_bwd_grid(int M) {
-  int g = (M + 1) / 2;
+// Rows per block of the LN backward: 256 threads, WPR = 8 / groups warps per row (the H = 768 kernel: 3 x 2 warps).
+static inline int ln_bwd_groups(int H) { return H <= 256 ? 8 : (H <= 512 ? 4 : (H <= 1024 ? 2 : 1)); }
+// ~80 registers x 256 threads -> 3 blocks per SM are co-resident; one exact wave (a grid of 4 per SM ran a 1/3-full
+// second wave).  The per-block partial column sums are sized by the same grid.
+static inline int ln_bwd_grid(int M, int H) {
+  const int g = (M + ln_bwd_groups(H) - 1) / ln_bwd_groups(H);
   return g < num_sms() * 3 ? g : num_sms() * 3;
 }
 
-int ln_bwd_workspace_floats(int M, int H) { return ln2_grid(M) * 3 * H; }
+int ln_bwd_workspace_floats(int M, int H) { return ln_bwd_grid(M, H) * 3 * H; }
 
 void layer_norm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const float* gamma, void* dx,
                     void* dxd, float* dgamma, float* dbeta, float* dbias, float* workspace, int M, int H,
@@ -1036,35 +779,27 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
                     cudaStream_t st, const uint8_t* keep_mask) {
   unsigned int th; float sc;
   drop_params(p_drop, th, sc);
-  static const int split = []() {
-    const char* e = getenv("B200_LN_FINALIZE_SPLIT");
-    const int z = e ? atoi(e) : 8;
-    return z < 1 ? 1 : (z > 32 ? 32 : z);
-  }();
-  if (ln_fast_enabled() && f8.q == nullptr && (in_stream == 0xFFFFFFFFu || th == 0) && H % 256 == 0 && H <= 1024) {
-    const __nv_bfloat16 *dyp = (const __nv_bfloat16*)dy, *xp = (const __nv_bfloat16*)x;
-    __nv_bfloat16 *dxp = (__nv_bfloat16*)dx, *dxdp = (__nv_bfloat16*)dxd;
-    const int wpr = H / 256;
-    const int groups = wpr == 4 ? 2 : (wpr == 3 ? 2 : (wpr == 2 ? 4 : 8));
-    int g = (M + groups - 1) / groups;
-    const int cap = ln2_bwd_grid(M);     // the workspace is sized for ln2_grid(M) >= this
-    if (g > cap) g = cap;
-    switch (wpr) {
-      case 1: launch_pdl(ln_bwd3_kernel<1, 8>, dim3(g), dim3(256), 0, st, dyp, xp, mean, rstd, gamma, dxp, dxdp, workspace, M, seed, drop_stream, th, sc, keep_mask); break;
-      case 2: launch_pdl(ln_bwd3_kernel<2, 4>, dim3(g), dim3(256), 0, st, dyp, xp, mean, rstd, gamma, dxp, dxdp, workspace, M, seed, drop_stream, th, sc, keep_mask); break;
-      case 3: launch_pdl(ln_bwd3_kernel<3, 2>, dim3(g), dim3(192), 0, st, dyp, xp, mean, rstd, gamma, dxp, dxdp, workspace, M, seed, drop_stream, th, sc, keep_mask); break;
-      default: launch_pdl(ln_bwd3_kernel<4, 2>, dim3(g), dim3(256), 0, st, dyp, xp, mean, rstd, gamma, dxp, dxdp, workspace, M, seed, drop_stream, th, sc, keep_mask); break;
-    }
-    dim3 g2((H + 31) / 32, 3, split);
-    launch_pdl(colsum_finalize_kernel, g2, dim3(256), 0, st, (const float*)workspace, g, H, dgamma, dbeta, dxd ? dbias : (float*)nullptr);
-    return;
+  decltype(&ln_bwd3_kernel<1, 8, false, false>) k;
+  int wpr;
+  if (f8.q == nullptr && (in_stream == 0xFFFFFFFFu || th == 0) && H % 256 == 0 && H <= 1024) {   // the encoder LNs of the bf16 path
+    wpr = H / 256;
+    k = wpr == 1 ? ln_bwd3_kernel<1, 8, false, false> : wpr == 2 ? ln_bwd3_kernel<2, 4, false, false>
+      : wpr == 3 ? ln_bwd3_kernel<3, 2, false, false> : ln_bwd3_kernel<4, 2, false, false>;
+  } else {
+    wpr = 8 / ln_bwd_groups(H);
+    if (f8.q == nullptr)
+      k = wpr == 1 ? ln_bwd3_kernel<1, 8, true, false> : wpr == 2 ? ln_bwd3_kernel<2, 4, true, false>
+        : wpr == 4 ? ln_bwd3_kernel<4, 2, true, false> : ln_bwd3_kernel<8, 1, true, false>;
+    else
+      k = wpr == 1 ? ln_bwd3_kernel<1, 8, true, true> : wpr == 2 ? ln_bwd3_kernel<2, 4, true, true>
+        : wpr == 4 ? ln_bwd3_kernel<4, 2, true, true> : ln_bwd3_kernel<8, 1, true, true>;
   }
-  const int grid = ln2_bwd_grid(M);
-  DISPATCH_WPR(H, (ln_bwd2_kernel<WPR><<<grid, 2 * WPR * 32, 0, st>>>(
-      (const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, mean, rstd, gamma, (__nv_bfloat16*)dx, (__nv_bfloat16*)dxd,
-      workspace, M, H, seed, drop_stream, in_stream, th, sc, f8)));
-  dim3 g2((H + 31) / 32, 3, split);
-  launch_pdl(colsum_finalize_kernel, g2, dim3(256), 0, st, (const float*)workspace, grid, H, dgamma, dbeta, dxd ? dbias : (float*)nullptr);
+  const int grid = ln_bwd_grid(M, H);
+  launch_pdl(k, dim3(grid), dim3(wpr * ln_bwd_groups(H) * 32), 0, st, (const __nv_bfloat16*)dy,
+             (const __nv_bfloat16*)x, mean, rstd, gamma, (__nv_bfloat16*)dx, (__nv_bfloat16*)dxd, workspace, M, seed,
+             drop_stream, th, sc, keep_mask, H, in_stream, f8);
+  launch_pdl(colsum_finalize_kernel, dim3((H + 31) / 32, 3, 8), dim3(256), 0, st, (const float*)workspace, grid, H,
+             dgamma, dbeta, dxd ? dbias : (float*)nullptr);
 }
 
 // Keep bits of one hidden-dropout site, one byte per 8 elements ([M][N / 8], bit t of byte j = element 8 j + t kept):
@@ -1128,8 +863,7 @@ void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float
   const size_t work = (size_t)M * (H / 8);
   int grid = (int)((work + 255) / 256);
   if (grid > num_sms() * 16) grid = num_sms() * 16;
-  static const bool reduce_ok = []() { const char* e = getenv("B200_EMBED_REDUCE"); return !(e && e[0] == '0'); }();
-  if (reduce_ok && M % S == 0 && H % 8 == 0 && (gtype == nullptr || type_rows == 2)) {
+  if (M % S == 0 && H % 8 == 0 && (gtype == nullptr || type_rows == 2)) {
     // word rows: scatter with atomics (30 k rows, little contention); position / token-type rows: reductions
     embed_bwd_scatter_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)de, ids, seg, gword, nullptr, nullptr, M, S, H);
     dim3 g2((H + 255) / 256, (S + 7) / 8);

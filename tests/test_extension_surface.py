@@ -53,3 +53,21 @@ def test_tile_variant_heuristic_sends_the_bert_large_shapes_to_the_cta_pair_kern
     assert api.pick_block_n(1024, 1024) in (128, 256)
     # the narrow variant only when it wastes (clearly) fewer SM slots in the last wave
     assert api._pick_block_n(128, api.NUM_SMS * 128) == 128
+
+
+def test_layer_norm_bindings_reject_unsupported_widths():
+    """The LayerNorm kernels cover H % 8 == 0 up to 2048: any other width is a RuntimeError raised before anything is
+    launched (host tensors suffice), not a process abort."""
+    import torch
+    from bert_pytorch_b200.ops import _loader
+    if not os.path.exists(_loader.extension_path()):
+        pytest.skip("extension not built (python -m bert_pytorch_b200.ops.build)")
+    C = _loader.load_extension()
+    for H in (1028, 2056):
+        x = torch.zeros(4, H, dtype=torch.bfloat16)
+        g, stats = torch.ones(H), torch.zeros(4)
+        with pytest.raises(RuntimeError, match="hidden size"):
+            C.layer_norm_fwd(x, g, g, torch.empty_like(x), stats, stats, 1e-12, None, None, False)
+        with pytest.raises(RuntimeError, match="hidden size"):
+            C.layer_norm_bwd(x, x, stats, stats, g, torch.empty_like(x), None, None, None, None, torch.zeros(1), 0.0, 0,
+                             0, 0xFFFFFFFF, None, None, False, None)

@@ -120,16 +120,17 @@ def test_fp8_engine_tracks_bf16_engine():
 
 def test_producer_kernels_emit_fp8_copies():
     """LayerNorm fwd/bwd, GELU and dGELU write the fp8 copy of their output in the same pass (delayed scaling):
-    the copy must dequantise to the bf16 output and the amax record must see the tensor."""
+    the copy must dequantise to the bf16 output and the amax record must see the tensor.  LayerNorm also at a width
+    that is not a multiple of 256 (128: the tiny models)."""
     ops = _ops()
     api = ops.api
     dev = torch.device("cuda")
     M, H = 512, 1024
     x = torch.randn(M, H, device=dev).bfloat16()
     g, b = torch.rand(H, device=dev) + 0.5, torch.randn(H, device=dev) * 0.1
-    meta = api.Fp8Meta(["ln", "gelu", "dxd", "dgelu"], [False, False, True, True], dev)
-    # scales as the previous step would have left them
-    for site, t in (("ln", 16.0), ("gelu", 8.0), ("dxd", 0.25), ("dgelu", 0.25)):      # generous: nothing saturates
+    meta = api.Fp8Meta(["ln", "gelu", "dxd", "dgelu", "ln128", "dxd128"], [False, False, True, True, False, True], dev)
+    # scales as the previous step would have left them (generous: nothing saturates)
+    for site, t in (("ln", 16.0), ("gelu", 8.0), ("dxd", 0.25), ("dgelu", 0.25), ("ln128", 16.0), ("dxd128", 0.25)):
         rec = meta.record(site)
         rec[0] = t
     meta.update()
@@ -153,6 +154,13 @@ def test_producer_kernels_emit_fp8_copies():
     dbi = torch.zeros(H, device=dev)
     d1, q = api.dgelu_bwd(dy, x, dbi, fp8=(meta, "dgelu"))
     close(q, d1, "dgelu", 0.14)
+    xt, gt, bt, dyt = x[:, :128].contiguous(), g[:128].contiguous(), b[:128].contiguous(), dy[:, :128].contiguous()
+    y, mean, rstd, q = api.layer_norm_fwd(xt, gt, bt, fp8=(meta, "ln128"))
+    close(q, y, "ln128", 0.07)
+    dg, db, dbias = (torch.zeros(128, device=dev) for _ in range(3))
+    dx, dxd, q = api.layer_norm_bwd(dyt, xt, mean, rstd, gt, dgamma=dg, dbeta=db, dbias=dbias, want_dropped=True,
+                                    p_drop=0.1, seed=11, drop_stream=3, fp8=(meta, "dxd128"))
+    close(q, dxd, "dxd128", 0.14)
 
 
 def test_attention_kernels_emit_fp8_copies():

@@ -16,7 +16,7 @@ def _api():
     return api
 
 
-@pytest.mark.parametrize("M,H", [(64, 64), (1000, 1024), (300, 768), (130, 256)])
+@pytest.mark.parametrize("M,H", [(64, 64), (1000, 1024), (300, 768), (130, 256), (257, 128), (300, 320), (200, 2048)])
 def test_layer_norm_fwd_bwd(M, H):
     K = _api()
     x = (torch.randn(M, H, device="cuda") * 2 + 0.5).to(torch.bfloat16)
@@ -36,6 +36,31 @@ def test_layer_norm_fwd_bwd(M, H):
     assert torch.allclose(dg, gr.grad, rtol=2e-2, atol=2e-1)
     assert torch.allclose(db, br.grad, rtol=2e-2, atol=2e-1)
     assert torch.allclose(dbias, dx.float().sum(0), rtol=2e-2, atol=2e-1)
+
+
+@pytest.mark.parametrize("M,H", [(512, 1024), (200, 320)])
+def test_layer_norm_bwd_input_dropout(M, H):
+    """``in_stream`` (the embedding LN, whose output was dropped out): dy is first multiplied by the keep decisions of
+    that stream, element index row * H + col, and by the kept-element scale -- against an fp32 reference fed the same
+    mask from the host twin of the generator."""
+    K = _api()
+    from bert_pytorch_b200.utils import philox
+    p, seed, stream = 0.1, 1234, 1023 * 8
+    x = (torch.randn(M, H, device="cuda") * 2 + 0.5).to(torch.bfloat16)
+    g = torch.randn(H, device="cuda") * 0.5 + 1.0
+    b = torch.randn(H, device="cuda") * 0.1
+    dy = torch.randn(M, H, device="cuda").to(torch.bfloat16)
+    y, mean, rstd = K.layer_norm_fwd(x, g, b)
+    keep = torch.from_numpy(philox.keep_mask(seed, stream, M * H, p)).view(M, H).cuda()
+    xr = x.float().requires_grad_(True)
+    gr, br = g.clone().requires_grad_(True), b.clone().requires_grad_(True)
+    F.layer_norm(xr, (H,), gr, br, eps=1e-12).backward(dy.float() * keep * philox.keep_scale(p))
+    dg, db = torch.zeros(H, device="cuda"), torch.zeros(H, device="cuda")
+    dx, dxd = K.layer_norm_bwd(dy, x, mean, rstd, g, dgamma=dg, dbeta=db, p_drop=p, seed=seed, in_stream=stream)
+    assert dxd is None
+    assert (dx.float() - xr.grad).abs().max() < 3e-2 * max(1.0, xr.grad.abs().max().item())
+    assert torch.allclose(dg, gr.grad, rtol=2e-2, atol=2e-1)
+    assert torch.allclose(db, br.grad, rtol=2e-2, atol=2e-1)
 
 
 def test_layer_norm_dropout_mask_consistency():
