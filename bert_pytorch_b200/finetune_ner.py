@@ -45,6 +45,9 @@ def parse_arguments(argv=None):
     p.add_argument("--seed", type=int, default=42)
     p.add_argument("--no_cuda", action="store_true")
     p.add_argument("--bf16", action="store_true", help="bf16 compute through the fused engine (new)")
+    p.add_argument("--unpad", action="store_true", default=False,
+                   help="with --bf16: the fused engine computes only the unmasked tokens, in training and evaluation "
+                        "(exact: the loss and F1 read unmasked positions only) (new)")
     args = p.parse_args(argv)
     args.cuda = torch.cuda.is_available() and not args.no_cuda
     return args
@@ -157,6 +160,7 @@ def main(argv=None) -> Dict[str, float]:
     model.to(dev)
     if not (args.cuda and args.bf16):
         model.bert.use_fused = False          # fp32 requested: plain PyTorch path
+    model.bert.unpad = bool(args.unpad)
     arena = ParamArena(model, device=dev)
     optimizer = Adam(model.parameters(), lr=args.lr, bias_correction=False)
     arena.bind_optimizer(optimizer)

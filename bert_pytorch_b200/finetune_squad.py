@@ -96,6 +96,10 @@ def build_parser() -> argparse.ArgumentParser:
     # new
     p.add_argument("--bf16", default=False, action="store_true")
     p.add_argument("--backend", default=None, choices=[None, "nccl", "gloo", "fused"])
+    p.add_argument("--unpad", default=False, action="store_true",
+                   help="prediction through the fused engine computes only the unmasked tokens. Training stays padded: "
+                        "the start / end cross-entropy normalises over every position, padded ones included, so an "
+                        "unpadded training step would not be exact")
     return p
 
 
@@ -316,6 +320,7 @@ def main(argv=None) -> dict:
         data = _features_to_tensors(eval_features, False)
         loader = DataLoader(data, sampler=SequentialSampler(data), batch_size=args.predict_batch_size)
         model.eval()
+        model.bert.unpad = bool(args.unpad)
         results: List[SQ.RawResult] = []
         t0 = time.time()
         with torch.no_grad():

@@ -26,11 +26,17 @@ Activations are saved rather than recomputed by default: an H100 has 80 GB (phas
 ~10 GB); ``--checkpoint_activations`` replays ceil(sqrt(L))-layer segments instead.
 Options: fp8 GEMM operands (``enable_fp8`` / ``B200_FP8=1`` / ``--fp8``), whole-micro-step CUDA-graph replay
 (``FusedPretrainer``, on by default, ``B200_GRAPH=0`` disables), K-FAC taps.
+
+Unpadded mode (``BertModel.unpad``, fine-tuning and inference through :meth:`FusedEncoderEngine.encode`): the
+unmasked tokens of the [B, S] batch are packed into T rows (:func:`pack_rows`) and every kernel runs on those rows
+only -- embeddings with explicit position ids, GEMMs / LayerNorms / dropout with M = T, variable-length attention
+over ``cu_seqlens``.  The output is scattered back into a zeroed [B*S, H] tensor.
 """
 from __future__ import annotations
 
 import math
 import os
+import warnings
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
@@ -83,9 +89,31 @@ class _LayerSaved:
 
 
 @dataclass
+class Packing:
+    """The unmasked tokens of a [B, S] batch packed back to back (one record per call, shared by every layer)."""
+    rows: torch.Tensor          # int32 [T]: index b * S + s of every unmasked token, in order
+    cu_seqlens: torch.Tensor    # int32 [B + 1]: sequence b is packed rows cu_seqlens[b] .. cu_seqlens[b + 1]
+    pos_ids: torch.Tensor       # int32 [T]: position s of every packed row
+    T: int
+    S: int
+
+
+def pack_rows(attention_mask: torch.Tensor) -> Packing:
+    """Packing of any 0/1 ``attention_mask`` [B, S] (holes included).  ``torch.nonzero`` costs one host sync."""
+    B, S = attention_mask.shape
+    keep = attention_mask != 0
+    rows = torch.nonzero(keep.reshape(-1)).squeeze(1)
+    cu = torch.zeros(B + 1, dtype=torch.int32, device=attention_mask.device)
+    cu[1:] = torch.cumsum(keep.sum(dim=1, dtype=torch.int32), 0, dtype=torch.int32)
+    return Packing(rows=rows.to(torch.int32), cu_seqlens=cu, pos_ids=(rows % S).to(torch.int32),
+                   T=rows.numel(), S=S)
+
+
+@dataclass
 class _Saved:
     B: int = 0
     S: int = 0
+    pk: Optional[Packing] = None
     seed: int = 0
     p_hidden: float = 0.0
     p_attn: float = 0.0
@@ -294,11 +322,13 @@ class FusedEncoderEngine:
     # -- forward --------------------------------------------------------------------------------
     @torch.no_grad()
     def forward(self, input_ids, token_type_ids, attention_mask, training: bool, seed: Optional[int] = None,
-                dropout: Optional[bool] = None):
+                dropout: Optional[bool] = None, pack: Optional[Packing] = None):
         """Returns (sequence_output [B*S, H] bf16, saved-or-None).  ``training`` saves activations for
-        ``backward``; ``dropout`` (default: same as ``training``) applies the dropout sites."""
+        ``backward``; ``dropout`` (default: same as ``training``) applies the dropout sites.  With ``pack``
+        (:func:`pack_rows` of the mask, at least one token) only the packed rows are computed: the sequence output is
+        [T, H] and the dropout elements are counted by packed row."""
         B, S = input_ids.shape
-        M, H, A = B * S, self.H, self.arena
+        H, A = self.H, self.arena
         dropout = training if dropout is None else dropout
         ph = self.p_hidden if dropout else 0.0
         pa = self.p_attn if dropout else 0.0
@@ -308,14 +338,19 @@ class FusedEncoderEngine:
         if self.has_type:
             seg = (token_type_ids if token_type_ids is not None else torch.zeros_like(input_ids)
                    ).reshape(-1).to(torch.int32).contiguous()
-        seqlens = attention_mask.to(torch.int32).sum(dim=1, dtype=torch.int32).contiguous()
-        sv = _Saved(B=B, S=S, seed=seed, p_hidden=ph, p_attn=pa, ids=ids, seg=seg, seqlens=seqlens) if training else None
+        if pack is not None:
+            ids = ids.index_select(0, pack.rows)
+            seg = seg.index_select(0, pack.rows) if seg is not None else None
+            seqlens = None
+        else:
+            seqlens = attention_mask.to(torch.int32).sum(dim=1, dtype=torch.int32).contiguous()
+        sv = _Saved(B=B, S=S, pk=pack, seed=seed, p_hidden=ph, p_attn=pa, ids=ids, seg=seg, seqlens=seqlens) if training else None
 
         x, e, mean, rstd = K.embedding_fwd(
             ids, seg, self.w("embeddings.word_embeddings.weight"), self.w("embeddings.position_embeddings.weight"),
             self.w("embeddings.token_type_embeddings.weight") if self.has_type else None,
             self.p("embeddings.LayerNorm.weight"), self.p("embeddings.LayerNorm.bias"), S,
-            p_drop=ph, seed=seed, stream=_stream(_EMB_LAYER, SITE_EMB))
+            p_drop=ph, seed=seed, stream=_stream(_EMB_LAYER, SITE_EMB), pos_ids=pack.pos_ids if pack is not None else None)
         if training:
             sv.emb_sum, sv.emb_mean, sv.emb_rstd = e, mean, rstd
 
@@ -327,16 +362,18 @@ class FusedEncoderEngine:
             if ckpt and l % seg_len == 0:
                 sv.boundaries[l] = x             # --checkpoint_activations: keep segment inputs only (K27)
             x, ls, xq = self._layer_forward(l, x, seqlens, B, S, ph, pa, seed, save=training and not ckpt,
-                                            xq=None if (l == 0 or (ckpt and l % seg_len == 0)) else xq)
+                                            xq=None if (l == 0 or (ckpt and l % seg_len == 0)) else xq, pk=pack)
             if ls is not None:
                 sv.layers.append(ls)
         if ckpt:
             sv.seg_len = seg_len
         return x, sv
 
-    def _layer_forward(self, l: int, x, seqlens, B: int, S: int, ph: float, pa: float, seed: int, save: bool, xq=None):
-        """One post-LN transformer layer (reference: src/modeling.py:482-499) as 9 kernel launches."""
-        A, H, M = self.arena, self.H, B * S
+    def _layer_forward(self, l: int, x, seqlens, B: int, S: int, ph: float, pa: float, seed: int, save: bool, xq=None,
+                       pk: Optional[Packing] = None):
+        """One post-LN transformer layer (reference: src/modeling.py:482-499) as 9 kernel launches.  ``x``: [B*S, H],
+        or [T, H] packed rows with ``pk``."""
+        A, H, M = self.arena, self.H, x.size(0)
         training = save or pa > 0 or ph > 0
         pre = f"encoder.layer.{l}."
         ls = _LayerSaved() if save else None
@@ -347,6 +384,10 @@ class FusedEncoderEngine:
             ctx_q = None
             if save:
                 ls.sdpa = sd
+        elif pk is not None:
+            ctx, lse = K.attention_fwd(qkv, None, self.heads, p_drop=pa, seed=seed, stream=_stream(l, SITE_ATTN_PROB),
+                                       cu_seqlens=pk.cu_seqlens, S=S)
+            ctx_q = None
         else:
             ctx, lse, *q = K.attention_fwd(qkv.view(B, S, 3 * H), seqlens, self.heads, p_drop=pa, seed=seed,
                                            stream=_stream(l, SITE_ATTN_PROB), fp8=self._side(f"{l}.ctx"))
@@ -398,9 +439,9 @@ class FusedEncoderEngine:
     # -- backward -------------------------------------------------------------------------------
     @torch.no_grad()
     def backward(self, sv: _Saved, d_out: torch.Tensor) -> None:
-        """``d_out``: [B*S, H] bf16 gradient of the sequence output.  Accumulates every parameter
-        gradient of the encoder into the arena."""
-        A, H, M = self.arena, self.H, sv.B * sv.S
+        """``d_out``: [B*S, H] bf16 gradient of the sequence output ([T, H] packed rows when the forward ran with a
+        packing).  Accumulates every parameter gradient of the encoder into the arena."""
+        A, H = self.arena, self.H
         ph, pa, seed = sv.p_hidden, sv.p_attn, sv.seed
         d = d_out
         kfac = getattr(self.bert, "_kfac", None)      # K-FAC taps: the saved activations double as its statistics
@@ -411,7 +452,7 @@ class FusedEncoderEngine:
                 hi = min(self.L, lo + sv.seg_len)
                 x, saved, xq = sv.boundaries.pop(lo), [], None
                 for l in range(lo, hi):                   # same seed -> same Philox dropout masks as the first pass
-                    x, ls, xq = self._layer_forward(l, x, sv.seqlens, sv.B, sv.S, ph, pa, seed, save=True, xq=xq)
+                    x, ls, xq = self._layer_forward(l, x, sv.seqlens, sv.B, sv.S, ph, pa, seed, save=True, xq=xq, pk=sv.pk)
                     saved.append(ls)
                 for l in reversed(range(lo, hi)):
                     d = self._layer_backward(l, saved[l - lo], d, sv, kfac)
@@ -427,14 +468,15 @@ class FusedEncoderEngine:
             p_drop=ph, seed=seed, in_stream=_stream(_EMB_LAYER, SITE_EMB) if ph > 0 else K.NO_STREAM)
         K.embedding_bwd_scatter(d_e, sv.ids, sv.seg, self.g("embeddings.word_embeddings.weight"),
                                 self.g("embeddings.position_embeddings.weight"),
-                                self.g("embeddings.token_type_embeddings.weight") if self.has_type else None, sv.S)
+                                self.g("embeddings.token_type_embeddings.weight") if self.has_type else None, sv.S,
+                                pos_ids=sv.pk.pos_ids if sv.pk is not None else None)
         self._join_wgrads()
         if self.fp8:                       # delayed scaling: next micro-step quantises with this one's amaxes
             self.meta.update()
             self._fp8_calibrated = True
 
     def _layer_backward(self, l: int, ls: _LayerSaved, d: torch.Tensor, sv: _Saved, kfac) -> torch.Tensor:
-        A, H, M = self.arena, self.H, sv.B * sv.S
+        A, H, M = self.arena, self.H, d.size(0)
         ph, pa, seed = sv.p_hidden, sv.p_attn, sv.seed
         pre = f"encoder.layer.{l}."
         # ---- LN2 -> (residual grad, dropped grad of the FFN-2 output)
@@ -478,6 +520,9 @@ class FusedEncoderEngine:
         dqkv_q = None
         if ls.sdpa is not None:
             d_qkv = self._sdpa_bwd(ls.sdpa, d_ctx, sv.B, sv.S)
+        elif sv.pk is not None:
+            d_qkv = K.attention_bwd(ls.qkv, None, ls.ctx, d_ctx, ls.lse, self.heads, p_drop=pa, seed=seed,
+                                    stream=_stream(l, SITE_ATTN_PROB), cu_seqlens=sv.pk.cu_seqlens, S=sv.S)
         else:
             d_qkv, *q = _as_tuple(K.attention_bwd(ls.qkv.view(sv.B, sv.S, 3 * H), sv.seqlens, ls.ctx.view(sv.B, sv.S, H),
                                                   d_ctx.view(sv.B, sv.S, H), ls.lse, self.heads, p_drop=pa, seed=seed,
@@ -517,32 +562,59 @@ class FusedEncoderEngine:
         return torch.stack([dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2)], dim=2).reshape(B * S, 3 * H)
 
     # -- autograd bridge for models with ordinary torch heads (finetuning, inference) ------------------
+    def _packing(self, attention_mask) -> Optional[Packing]:
+        """The packing of this batch when ``BertModel.unpad`` is set and the unpadded path can serve the engine's
+        configuration (fp8 operands and the library attention run padded), else None."""
+        if not getattr(self.bert, "unpad", False):
+            return None
+        if self.fp8 or _use_sdpa():
+            if not getattr(self, "_unpad_warned", False):
+                warnings.warn("BertModel.unpad: fp8 operands and B200_ATTN=sdpa have no unpadded path; running padded")
+                self._unpad_warned = True
+            return None
+        return pack_rows(attention_mask)
+
     def encode(self, input_ids, token_type_ids, attention_mask) -> torch.Tensor:
         B, S = input_ids.shape
         training = self.bert.training and torch.is_grad_enabled()
-        if not training:
-            seq, _ = self.forward(input_ids, token_type_ids, attention_mask, training=False)
-            out = seq.view(B, S, self.H)
+        pack = self._packing(attention_mask)
+        if pack is not None and pack.T == 0:          # nothing to compute: the output at masked positions is zero
+            out = torch.zeros(B, S, self.H, dtype=torch.bfloat16, device=input_ids.device)
+        elif not training:
+            seq, _ = self.forward(input_ids, token_type_ids, attention_mask, training=False, pack=pack)
+            out = _unpack(seq, pack, B * S).view(B, S, self.H)
         else:
-            out = _EncoderFn.apply(self._hook, self, input_ids, token_type_ids, attention_mask)
+            out = _EncoderFn.apply(self._hook, self, input_ids, token_type_ids, attention_mask, pack)
         if torch.is_autocast_enabled():
             return out.to(torch.get_autocast_dtype("cuda"))
         return out.float()
 
 
+def _unpack(seq: torch.Tensor, pack: Optional[Packing], rows: int) -> torch.Tensor:
+    """Packed rows [T, H] -> [rows, H] with zeros at the masked positions (identity without a packing)."""
+    if pack is None:
+        return seq
+    out = torch.zeros(rows, seq.size(1), dtype=seq.dtype, device=seq.device)
+    K.scatter_rows(seq, pack.rows, out)
+    return out
+
+
 class _EncoderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, hook, engine, input_ids, token_type_ids, attention_mask):
-        seq, sv = engine.forward(input_ids, token_type_ids, attention_mask, training=True)
+    def forward(ctx, hook, engine, input_ids, token_type_ids, attention_mask, pack=None):
+        seq, sv = engine.forward(input_ids, token_type_ids, attention_mask, training=True, pack=pack)
         ctx.engine, ctx.sv = engine, sv
-        return seq.view(input_ids.size(0), input_ids.size(1), engine.H)
+        return _unpack(seq, pack, input_ids.numel()).view(input_ids.size(0), input_ids.size(1), engine.H)
 
     @staticmethod
     def backward(ctx, d_seq):
         engine, sv = ctx.engine, ctx.sv
-        engine.backward(sv, d_seq.reshape(-1, engine.H).to(torch.bfloat16).contiguous())
+        d = d_seq.reshape(-1, engine.H).to(torch.bfloat16).contiguous()
+        if sv.pk is not None:                       # the gradient of the packed rows; masked positions had no effect
+            d = K.gather_rows(d, sv.pk.rows)
+        engine.backward(sv, d)
         ctx.sv = None
-        return torch.zeros(1, device=d_seq.device), None, None, None, None
+        return torch.zeros(1, device=d_seq.device), None, None, None, None, None
 
 
 class _HeadLinearFn(torch.autograd.Function):

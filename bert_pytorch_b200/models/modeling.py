@@ -495,7 +495,16 @@ def load_tf_weights_in_bert(model: nn.Module, tf_checkpoint_path: str) -> nn.Mod
 
 
 class BertModel(BertPreTrainedModel):
-    """Embeddings + encoder (+ pooler iff ``next_sentence``) -- src/modeling.py:802-883."""
+    """Embeddings + encoder (+ pooler iff ``next_sentence``) -- src/modeling.py:802-883.
+
+    ``use_fused`` (default True): run the encoder through the sm_90a engine whenever it can.
+    ``unpad`` (default False): when the fused engine runs, compute only the tokens whose ``attention_mask`` is 1,
+    packed back to back, with variable-length attention over each sequence's tokens (any 0/1 mask, holes included).
+    The sequence output is then zero at positions where ``attention_mask == 0``; the padded engine computes those
+    positions as attention over the valid keys.  This is exact for every head that never reads masked positions --
+    token classification with its masked loss, sequence classification, multiple choice and QA prediction -- but not
+    for QA training, whose start / end cross-entropy normalises over all positions, masked ones included.
+    fp8 operands and ``B200_ATTN=sdpa`` have no unpadded path: they run padded (with a warning)."""
 
     def __init__(self, config: BertConfig):
         super().__init__(config)
@@ -504,6 +513,7 @@ class BertModel(BertPreTrainedModel):
         self.pooler = BertPooler(config) if getattr(config, "next_sentence", True) else None
         self.output_all_encoded_layers = bool(getattr(config, "output_all_encoded_layers", False))
         self.use_fused = True   # the sm_90a engine is used whenever it can be
+        self.unpad = False      # fused engine on the unmasked tokens only (see the class docstring)
         self._engine = None
         self.apply(self.init_bert_weights)
 

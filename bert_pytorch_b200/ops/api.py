@@ -171,14 +171,17 @@ def layer_norm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, *, 
     return (y, mean, rstd) if fp8 is None else (y, mean, rstd, q)
 
 
-_LN_WS: Dict[Tuple[int, int, int], torch.Tensor] = {}
+_LN_WS: Dict[Tuple[int, int], torch.Tensor] = {}
 
 
 def _ln_workspace(M: int, H: int, device: torch.device) -> torch.Tensor:
-    key = (device.index or 0, M, H)
+    """One workspace per (device, H), sized for the largest grid the LN backward launches (the grid stops growing at a
+    few CTAs per SM), so that any row count fits -- the unpadded engine sees a new M every batch.  Entries are never
+    replaced: captured CUDA graphs keep their pointers."""
+    key = (device.index or 0, H)
     ws = _LN_WS.get(key)
     if ws is None:
-        ws = torch.empty(extension().ln_bwd_workspace(M, H), dtype=torch.float32, device=device)
+        ws = torch.empty(extension().ln_bwd_workspace(1 << 30, H), dtype=torch.float32, device=device)
         _LN_WS[key] = ws
     return ws
 
@@ -238,19 +241,23 @@ def dgelu_bwd(dy: torch.Tensor, x: torch.Tensor, dbias: Optional[torch.Tensor] =
     return dx if fp8 is None else (dx, q)
 
 
-def embedding_fwd(ids, seg, word, pos, type_emb, gamma, beta, S: int, *, eps=1e-12, p_drop=0.0, seed=0, stream=0):
+def embedding_fwd(ids, seg, word, pos, type_emb, gamma, beta, S: int, *, eps=1e-12, p_drop=0.0, seed=0, stream=0,
+                  pos_ids: Optional[torch.Tensor] = None):
+    """``pos_ids`` (int32, one per id): the position row of every token, for packed rows of an unpadded batch;
+    without it token ``i`` sits at position ``i % S``."""
     M, H = ids.numel(), word.size(1)
     e = torch.empty(M, H, dtype=torch.bfloat16, device=ids.device)
     y = torch.empty_like(e)
     mean = torch.empty(M, dtype=torch.float32, device=ids.device)
     rstd = torch.empty_like(mean)
-    extension().embedding_fwd(ids, seg, word, pos, type_emb, gamma, beta, e, y, mean, rstd, S, eps, p_drop, seed, stream)
+    extension().embedding_fwd(ids, seg, word, pos, type_emb, gamma, beta, e, y, mean, rstd, S, eps, p_drop, seed, stream,
+                              pos_ids)
     _count()
     return y, e, mean, rstd
 
 
-def embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S: int) -> None:
-    extension().embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S)
+def embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S: int, *, pos_ids: Optional[torch.Tensor] = None) -> None:
+    extension().embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S, pos_ids)
     _count()
 
 
@@ -294,28 +301,46 @@ def softmax_ce_(logits: torch.Tensor, targets: torch.Tensor, count: torch.Tensor
     _count()
 
 
-def attention_fwd(qkv: torch.Tensor, seqlens: torch.Tensor, heads: int, *, p_drop=0.0, seed=0, stream=0, fp8=None):
-    """``fp8=(meta, site)``: the kernel also writes the fp8 copy of the context -> (ctx, lse, q)."""
-    B, S, H3 = qkv.shape
-    H = H3 // 3
-    ctx = torch.empty(B, S, H, dtype=torch.bfloat16, device=qkv.device)
+def _attn_shape(qkv: torch.Tensor, seqlens, cu_seqlens, S):
+    """(B, S, rows, H) of the padded form (qkv [B, S, 3H], ``seqlens`` int32 [B]) or of the varlen form (qkv packed
+    [T, 3H], ``cu_seqlens`` int32 [B + 1], ``S`` the padded length)."""
+    if cu_seqlens is None:
+        B, S, H3 = qkv.shape
+        return B, S, B * S, H3 // 3
+    if seqlens is not None or S is None:
+        raise ValueError("the varlen form takes cu_seqlens and S, and no seqlens")
+    return cu_seqlens.numel() - 1, int(S), qkv.size(0), qkv.size(-1) // 3
+
+
+def attention_fwd(qkv: torch.Tensor, seqlens: Optional[torch.Tensor], heads: int, *, p_drop=0.0, seed=0, stream=0,
+                  fp8=None, cu_seqlens: Optional[torch.Tensor] = None, S: Optional[int] = None):
+    """Padded form: qkv [B, S, 3H], valid keys of sequence b = its first ``seqlens[b]`` -> ctx [B, S, H].
+    Varlen form (``cu_seqlens``, ``S``, ``seqlens=None``): qkv packed [T, 3H], sequence b = rows cu_seqlens[b] ..
+    cu_seqlens[b + 1] -> ctx [T, H]; ``S`` is the padded length (at most 512, a multiple of 8), which sizes the grid
+    and lse, and strides the dropout counter, so the keep decisions are the padded call's.  lse is [B, heads, S] in
+    both forms.  ``fp8=(meta, site)`` (padded form only): the kernel also writes the fp8 copy of the context ->
+    (ctx, lse, q)."""
+    B, S, rows, H = _attn_shape(qkv, seqlens, cu_seqlens, S)
+    ctx = torch.empty(*qkv.shape[:-1], H, dtype=torch.bfloat16, device=qkv.device)
     lse = torch.empty(B, heads, S, dtype=torch.float32, device=qkv.device)
     q, rec, e5 = _fp8_side(fp8, ctx)
-    extension().attention_fwd(qkv, seqlens, ctx, lse, heads, 1.0 / math.sqrt(H // heads), p_drop, seed, stream, q, rec, e5)
+    extension().attention_fwd(qkv, seqlens, ctx, lse, heads, 1.0 / math.sqrt(H // heads), p_drop, seed, stream, q, rec, e5,
+                              cu_seqlens, S)
     _count()
     return (ctx, lse) if fp8 is None else (ctx, lse, q)
 
 
-def attention_bwd(qkv, seqlens, ctx, dctx, lse, heads: int, *, p_drop=0.0, seed=0, stream=0, fp8=None):
-    """``fp8=(meta, site)``: the kernels also write the fp8 copy of dqkv -> (dqkv, q)."""
-    B, S, H3 = qkv.shape
-    H = H3 // 3
+def attention_bwd(qkv, seqlens, ctx, dctx, lse, heads: int, *, p_drop=0.0, seed=0, stream=0, fp8=None,
+                  cu_seqlens: Optional[torch.Tensor] = None, S: Optional[int] = None):
+    """Both forms as :func:`attention_fwd`.  ``fp8=(meta, site)``: the kernels also write the fp8 copy of dqkv ->
+    (dqkv, q)."""
+    B, S, rows, H = _attn_shape(qkv, seqlens, cu_seqlens, S)
     dqkv = torch.empty_like(qkv)
     delta = torch.empty(B, heads, S, dtype=torch.float32, device=qkv.device)
-    dq_acc = torch.empty(B * S, H, dtype=torch.float32, device=qkv.device)
+    dq_acc = torch.empty(rows, H, dtype=torch.float32, device=qkv.device)
     q, rec, e5 = _fp8_side(fp8, dqkv)
     extension().attention_bwd(qkv, seqlens, ctx, dctx, lse, dqkv, delta, dq_acc, heads, 1.0 / math.sqrt(H // heads), p_drop,
-                              seed, stream, q, rec, e5)
+                              seed, stream, q, rec, e5, cu_seqlens, S)
     _count(2)
     return dqkv if fp8 is None else (dqkv, q)
 

@@ -13,6 +13,12 @@
 //           formed in registers; dQ += dS K takes dS from registers; P~ and dS pass through shared memory once and
 //           are read MN-major for dV += P~^T dO and dK += dS^T Q.  dQ is reduced across key blocks with fp32 reductions
 //           into dq_acc and converted to bf16 by attn_dq_convert_kernel; delta = <dO, O> comes from attn_delta_kernel.
+// Varlen (VARLEN = true): qkv is packed [T, 3H] and ctx / dctx / dq_acc are [T, H]; sequence b owns rows
+// cu_seqlens[b] .. cu_seqlens[b + 1] (passed in AttnArgs::seqlens).  S is the padded length: it sizes the grid and is
+// the stride of the dropout counter, so the keep decisions equal the padded kernel's for the same batch.  lse and
+// delta stay [B, h, S], indexed by the position inside the sequence.  CTAs whose query block (forward) or key block
+// (backward) starts at or past the sequence's end exit at once; TMA boxes that run into the next sequence (or past T,
+// zero fill) are masked as keys, and every store is bounded by the sequence length so no neighbour row is written.
 // Dropout: Philox counter RNG, one draw per 8 consecutive keys of a (batch, head, query) row; the backward regenerates
 // the forward's keep decisions.  A draw serves the four lanes of a quad (each owns two of the eight keys): lane c of
 // the quad draws for key groups c, 4 + c, ... and quad_transpose hands every lane its 32-bit word of each draw.
@@ -118,15 +124,24 @@ __device__ __forceinline__ void store_tile64(const float (&acc)[32], float mul_l
 // ------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------
+template <bool VARLEN>
 __global__ void __launch_bounds__(128)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv, const AttnArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int qb = blockIdx.x, bh = blockIdx.y;
   const int b = bh / p.h, head = bh % p.h;
-  const int seqlen = min(p.seqlens[b], p.S);
+  int seqlen, row0;
+  if constexpr (VARLEN) {
+    pdl_wait();                                         // cu_seqlens may come from the previous kernel
+    row0 = p.seqlens[b];
+    seqlen = min(p.seqlens[b + 1] - row0, p.S);
+    if (qb * QT >= seqlen) return;                      // CTA uniform, before any mbarrier or TMA work
+  } else {
+    seqlen = min(p.seqlens[b], p.S);
+    row0 = b * p.S;
+  }
   const int nkb = max(1, (seqlen + KT - 1) / KT);       // key blocks that contain valid keys
-  const int row0 = b * p.S;
   uint8_t* sQ = smem;                                   // 8 KB
   uint8_t* sKV = smem + 8192;                           // per key block: K 16 KB | V 16 KB
   uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + (size_t)nkb * 32768);   // [0]: Q, [1 + j]: key block j
@@ -138,7 +153,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
+  if constexpr (!VARLEN) pdl_wait();
   pdl_trigger_small();
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(&bars[0], 8192);
@@ -240,29 +255,38 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   float amax = 0.f;
   const float qscale = p.f8.q ? p.f8.meta[1] : 0.f;
   const size_t tile_off = (size_t)(row0 + qb * QT) * p.H + head * HD;
-  store_tile64(o, 1.f / l[0], 1.f / l[1], r_lo, p.S - qb * QT, p.ctx + tile_off, (size_t)p.H, p.f8, tile_off, qscale, amax);
+  const int q_end = VARLEN ? seqlen : p.S;              // query rows that exist
+  store_tile64(o, 1.f / l[0], 1.f / l[1], r_lo, q_end - qb * QT, p.ctx + tile_off, (size_t)p.H, p.f8, tile_off, qscale, amax);
   if (p.f8.q) fp8_amax_commit(p.f8, amax);
   if (c == 0) {
 #pragma unroll
     for (int h = 0; h < 2; ++h)
-      if (q_lo + 8 * h < p.S) p.lse[(size_t)bh * p.S + q_lo + 8 * h] = (m[h] + log2f(l[h])) * 0.6931471805599453f;
+      if (q_lo + 8 * h < q_end) p.lse[(size_t)bh * p.S + q_lo + 8 * h] = (m[h] + log2f(l[h])) * 0.6931471805599453f;
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // backward
 // ------------------------------------------------------------------------------------------------
+template <bool VARLEN>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ dout, float* __restrict__ delta,
-                  int B, int S, int h, int H) {
-  // one 8-lane group per (token, head): 64 elements = 8 x 16 B
+                  int B, int S, int h, int H, const int* __restrict__ cu_seqlens) {
+  // one 8-lane group per (token, head): 64 elements = 8 x 16 B; varlen: per (sequence, position < seqlen, head)
   const long long gid = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
   const int sub = threadIdx.x & 7;
   const long long total = (long long)B * S * h;
   if (gid >= total) return;
   const int head = (int)(gid % h);
-  const long long tok = gid / h;
-  const size_t off = (size_t)tok * H + head * HD + sub * 8;
+  const long long tok = gid / h;                       // (sequence, position) of this group
+  long long row = tok;                                  // its row of o / dout
+  if constexpr (VARLEN) {
+    const int bb = (int)(tok / S), ss = (int)(tok % S);
+    const int r0 = cu_seqlens[bb];
+    if (ss >= cu_seqlens[bb + 1] - r0) return;
+    row = r0 + ss;
+  }
+  const size_t off = (size_t)row * H + head * HD + sub * 8;
   const uint4 a = *reinterpret_cast<const uint4*>(o + off), d = *reinterpret_cast<const uint4*>(dout + off);
   const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, dw[4] = {d.x, d.y, d.z, d.w};
   float s = 0.f;
@@ -271,9 +295,11 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __re
     const float2 x = unpack_bf16(aw[t]), y = unpack_bf16(dw[t]);
     s += x.x * y.x + x.y * y.y;
   }
-  s += __shfl_xor_sync(0xffffffffu, s, 1);
-  s += __shfl_xor_sync(0xffffffffu, s, 2);
-  s += __shfl_xor_sync(0xffffffffu, s, 4);
+  // varlen: groups past their sequence's end have returned, so each group reduces among its own 8 lanes only
+  const unsigned gm = VARLEN ? (0xFFu << (threadIdx.x & 24)) : 0xffffffffu;
+  s += __shfl_xor_sync(gm, s, 1);
+  s += __shfl_xor_sync(gm, s, 2);
+  s += __shfl_xor_sync(gm, s, 4);
   if (sub == 0) {
     const int bb = (int)(tok / S), ss = (int)(tok % S);
     delta[((size_t)bb * h + head) * S + ss] = s;
@@ -289,6 +315,7 @@ __device__ __forceinline__ uint32_t tile_pair_offset(int r, int g, int c) {
 constexpr int ATT_BWD_THREADS = 256;
 constexpr int ATT_BWD_SMEM = 16384 * 2 + 8192 * 8 + 1024 + 64;
 
+template <bool VARLEN>
 __global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
                 const __grid_constant__ CUtensorMap tmap_do, const AttnArgs p) {
@@ -304,9 +331,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
   const int kb = blockIdx.x, bh = blockIdx.y;
   const int b = bh / p.h, head = bh % p.h;
-  const int seqlen = min(p.seqlens[b], p.S);
-  const int row0 = b * p.S;
-  const int nqb = (p.S + QT - 1) / QT;
+  int seqlen, row0;
+  if constexpr (VARLEN) {
+    row0 = p.seqlens[b];
+    seqlen = min(p.seqlens[b + 1] - row0, p.S);
+    if (kb * KT >= seqlen) return;                      // CTA uniform, before any mbarrier or TMA work
+  } else {
+    seqlen = min(p.seqlens[b], p.S);
+    row0 = b * p.S;
+  }
+  const int q_end = VARLEN ? seqlen : p.S;              // query rows (and rows of dK / dV) that exist
+  const int nqb = (q_end + QT - 1) / QT;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_q);
@@ -365,7 +400,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = r_lo + 8 * h, q = i * QT + r;
-      const bool q_ok = q < p.S;
+      const bool q_ok = q < q_end;
       const float lse2 = q_ok ? __ldg(p.lse + (size_t)bh * p.S + q) * LOG2E : 0.f;
       const float dlt = q_ok ? __ldg(p.delta + (size_t)bh * p.S + q) : 0.f;
       uint32_t w[8];
@@ -413,7 +448,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int q = i * QT + r_lo + 8 * h;
-      if (q < p.S) {
+      if (q < q_end) {
         float* dst = p.dq_acc + (size_t)(row0 + q) * p.H + head * HD + 2 * c;
 #pragma unroll
         for (int g = 0; g < 8; ++g)
@@ -428,8 +463,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   float amax = 0.f;
   const float qscale = p.f8.q ? p.f8.meta[1] : 0.f;
   const size_t k_off = (size_t)(row0 + key0) * 3 * p.H + p.H + head * HD;
-  store_tile64(dk, 1.f, 1.f, r_lo, p.S - key0, p.dqkv + k_off, (size_t)3 * p.H, p.f8, k_off, qscale, amax);
-  store_tile64(dv, 1.f, 1.f, r_lo, p.S - key0, p.dqkv + k_off + p.H, (size_t)3 * p.H, p.f8, k_off + p.H, qscale, amax);
+  store_tile64(dk, 1.f, 1.f, r_lo, q_end - key0, p.dqkv + k_off, (size_t)3 * p.H, p.f8, k_off, qscale, amax);
+  store_tile64(dv, 1.f, 1.f, r_lo, q_end - key0, p.dqkv + k_off + p.H, (size_t)3 * p.H, p.f8, k_off + p.H, qscale, amax);
   if (p.f8.q) fp8_amax_commit(p.f8, amax);
 }
 
@@ -458,61 +493,75 @@ attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict_
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
+// head_dim 64, S <= 512 and S % 8 == 0 are checked by the bindings
 static void fill_args(AttnArgs& a, int B, int S, int h, int d, const int* seqlens, float scale,
                       Seed seed, unsigned int stream, float p_drop) {
-  if (d != HD) { fprintf(stderr, "[b200] attention kernels need head_dim 64 (got %d)\n", d); abort(); }
-  if (S > 512 || S % 8 != 0) { fprintf(stderr, "[b200] attention kernels need S <= 512 and S %% 8 == 0 (got %d)\n", S); abort(); }
   a.B = B; a.S = S; a.h = h; a.H = h * d; a.seqlens = seqlens; a.scale = scale; a.seed = seed; a.stream = stream;
   a.thresh16 = p_drop > 0.f ? (unsigned)(p_drop * 65536.f + 0.5f) : 0u;
   a.inv_keep = p_drop > 0.f ? 65536.f / (65536.f - (float)a.thresh16) : 1.f;
   a.ctx = nullptr; a.lse = nullptr; a.delta = nullptr; a.dqkv = nullptr; a.dq_acc = nullptr;
 }
 
-void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, int B, int S, int h, int d,
-                   float scale, Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st) {
-  AttnArgs a;
-  fill_args(a, B, S, h, d, seqlens, scale, seed, stream, p_drop);
-  a.ctx = (__nv_bfloat16*)ctx; a.lse = lse; a.f8 = f8;
-  const int H = h * d;
-  CUtensorMap tq = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)B * S, 3 * H, 64, QT);
-  CUtensorMap tkv = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)B * S, 3 * H, 64, KT);
+template <bool VARLEN>
+static void launch_fwd(const void* qkv, const AttnArgs& a, long long rows, cudaStream_t st) {
+  const int S = a.S, H = a.H;
+  CUtensorMap tq = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, QT);
+  CUtensorMap tkv = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, KT);
   const int nkb = (S + KT - 1) / KT;
   const int smem = 8192 + nkb * 32768 + 1024 + 64;
   static int configured = 0;
   if (smem > configured) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    B200_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = smem;
   }
-  launch_pdl(attn_fwd_kernel, dim3((S + QT - 1) / QT, B * h), dim3(128), (size_t)smem, st, tq, tkv, a);
+  launch_pdl(attn_fwd_kernel<VARLEN>, dim3((S + QT - 1) / QT, a.B * a.h), dim3(128), (size_t)smem, st, tq, tkv, a);
+}
+
+void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, int B, int S, int h, int d,
+                   float scale, Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
+                   const int* cu_seqlens, long long T) {
+  AttnArgs a;
+  fill_args(a, B, S, h, d, cu_seqlens ? cu_seqlens : seqlens, scale, seed, stream, p_drop);
+  a.ctx = (__nv_bfloat16*)ctx; a.lse = lse; a.f8 = f8;
+  if (cu_seqlens) launch_fwd<true>(qkv, a, T, st);
+  else launch_fwd<false>(qkv, a, (long long)B * S, st);
+}
+
+template <bool VARLEN>
+static void launch_bwd(const void* qkv, const void* ctx, const void* dctx, const AttnArgs& a, long long rows,
+                       cudaStream_t st) {
+  const int B = a.B, S = a.S, h = a.h, H = a.H;
+  const long long groups = (long long)B * S * h;
+  attn_delta_kernel<VARLEN><<<(unsigned)((groups * 8 + 255) / 256), 256, 0, st>>>(
+      (const __nv_bfloat16*)ctx, (const __nv_bfloat16*)dctx, const_cast<float*>(a.delta), B, S, h, H, a.seqlens);
+  B200_CUDA_CHECK(cudaMemsetAsync(a.dq_acc, 0, sizeof(float) * (size_t)rows * H, st));
+  CUtensorMap tq = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, QT);
+  CUtensorMap tkv = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, KT);
+  CUtensorMap td = make_tmap_2d_bf16(dctx, H, (uint64_t)rows, H, 64, QT);
+  static bool once = false;
+  if (!once) {
+    B200_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_BWD_SMEM));
+    once = true;
+  }
+  attn_bwd_kernel<VARLEN><<<dim3((S + KT - 1) / KT, B * h), ATT_BWD_THREADS, ATT_BWD_SMEM, st>>>(tq, tkv, td, a);
+  const long long work = rows * (H / 8);
+  int g = (int)((work + 255) / 256);
+  if (g > num_sms() * 16) g = num_sms() * 16;
+  attn_dq_convert_kernel<<<g, 256, 0, st>>>(a.dq_acc, a.dqkv, rows, H, a.f8);
 }
 
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
-                   Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st) {
+                   Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
+                   const int* cu_seqlens, long long T) {
   AttnArgs a;
-  fill_args(a, B, S, h, d, seqlens, scale, seed, stream, p_drop);
+  fill_args(a, B, S, h, d, cu_seqlens ? cu_seqlens : seqlens, scale, seed, stream, p_drop);
   a.f8 = f8;
-  const int H = h * d;
   a.lse = const_cast<float*>(lse); a.delta = delta_ws; a.dqkv = (__nv_bfloat16*)dqkv; a.dq_acc = dq_acc;
   a.ctx = (__nv_bfloat16*)const_cast<void*>(ctx);
   if (dq_acc == nullptr) { fprintf(stderr, "[b200] attention_bwd needs a dq accumulation buffer\n"); abort(); }
-  const long long groups = (long long)B * S * h;
-  attn_delta_kernel<<<(unsigned)((groups * 8 + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)ctx,
-                                                                       (const __nv_bfloat16*)dctx, delta_ws, B, S, h, H);
-  B200_CUDA_CHECK(cudaMemsetAsync(dq_acc, 0, sizeof(float) * (size_t)B * S * H, st));
-  CUtensorMap tq = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)B * S, 3 * H, 64, QT);
-  CUtensorMap tkv = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)B * S, 3 * H, 64, KT);
-  CUtensorMap td = make_tmap_2d_bf16(dctx, H, (uint64_t)B * S, H, 64, QT);
-  static bool once = false;
-  if (!once) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_BWD_SMEM));
-    once = true;
-  }
-  attn_bwd_kernel<<<dim3((S + KT - 1) / KT, B * h), ATT_BWD_THREADS, ATT_BWD_SMEM, st>>>(tq, tkv, td, a);
-  const long long work = (long long)B * S * (H / 8);
-  int g = (int)((work + 255) / 256);
-  if (g > num_sms() * 16) g = num_sms() * 16;
-  attn_dq_convert_kernel<<<g, 256, 0, st>>>(dq_acc, (__nv_bfloat16*)dqkv, (long long)B * S, H, a.f8);
+  if (cu_seqlens) launch_bwd<true>(qkv, ctx, dctx, a, T, st);
+  else launch_bwd<false>(qkv, ctx, dctx, a, (long long)B * S, st);
 }
 
 }  // namespace b200

@@ -251,9 +251,17 @@ void colsum(Tensor x, Tensor out) {
   b200::colsum_bf16(x.data_ptr(), (int)x.size(0), (int)x.size(1), (int)x.stride(0), out.data_ptr<float>(), cur_stream());
 }
 
+// pos_ids (optional int32 [M]): position of every token row (packed rows of an unpadded batch); else row % S
+inline const int* opt_pos_ids(const c10::optional<Tensor>& pos_ids, const Tensor& ids) {
+  if (!pos_ids.has_value() || !pos_ids->defined()) return nullptr;
+  TORCH_CHECK(pos_ids->scalar_type() == at::kInt && pos_ids->is_contiguous() && pos_ids->numel() == ids.numel() &&
+              pos_ids->device() == ids.device(), "pos_ids must be a contiguous int32 tensor like ids");
+  return pos_ids->data_ptr<int>();
+}
+
 void embedding_fwd(Tensor ids, c10::optional<Tensor> seg, Tensor word, Tensor pos, c10::optional<Tensor> type,
                    Tensor gamma, Tensor beta, Tensor e_out, Tensor y, Tensor mean, Tensor rstd, int64_t S, double eps,
-                   double p_drop, int64_t seed, int64_t stream_id) {
+                   double p_drop, int64_t seed, int64_t stream_id, c10::optional<Tensor> pos_ids) {
   TORCH_CHECK(ids.scalar_type() == at::kInt && ids.is_contiguous(), "ids must be contiguous int32");
   check_bf16(word, "word"); check_bf16(pos, "pos"); check_bf16(e_out, "e_out"); check_bf16(y, "y");
   const int H = (int)word.size(1), M = (int)ids.numel();
@@ -268,18 +276,19 @@ void embedding_fwd(Tensor ids, c10::optional<Tensor> seg, Tensor word, Tensor po
   b200::embedding_fwd(ids.data_ptr<int>(), seg_p, word.data_ptr(), pos.data_ptr(), type_p, gamma.data_ptr<float>(),
                       beta.data_ptr<float>(), e_out.data_ptr(), y.data_ptr(), mean.data_ptr<float>(),
                       rstd.data_ptr<float>(), M, (int)S, H, (float)eps, mk_seed(seed), (unsigned)stream_id,
-                      (float)p_drop, cur_stream());
+                      (float)p_drop, cur_stream(), opt_pos_ids(pos_ids, ids));
 }
 
 void embedding_bwd_scatter(Tensor de, Tensor ids, c10::optional<Tensor> seg, Tensor gword, Tensor gpos,
-                           c10::optional<Tensor> gtype, int64_t S) {
+                           c10::optional<Tensor> gtype, int64_t S, c10::optional<Tensor> pos_ids) {
   check_bf16(de, "de");
   const int H = (int)de.size(-1), M = (int)ids.numel();
   c10::cuda::CUDAGuard guard(de.device());
   b200::embedding_bwd_scatter(de.data_ptr(), ids.data_ptr<int>(),
                               seg.has_value() && seg->defined() ? seg->data_ptr<int>() : nullptr,
                               gword.data_ptr<float>(), gpos.data_ptr<float>(), opt_f32(gtype), M, (int)S, H,
-                              gtype.has_value() && gtype->defined() ? (int)gtype->size(0) : 0, cur_stream());
+                              gtype.has_value() && gtype->defined() ? (int)gtype->size(0) : 0, cur_stream(),
+                              opt_pos_ids(pos_ids, ids));
 }
 
 void mlm_compact(Tensor labels, int64_t max_pred, Tensor idx, Tensor tgt, Tensor count) {
@@ -365,26 +374,76 @@ void arena_adam(Tensor g, Tensor p, Tensor m, Tensor v, c10::optional<Tensor> sh
                    (float)beta2, (float)eps, (float)weight_decay, (int)step, bias_correction, adam_w_mode, cur_stream());
 }
 
-void attention_fwd(Tensor qkv, Tensor seqlens, Tensor ctx, Tensor lse, int64_t heads, double scale, double p_drop,
-                   int64_t seed, int64_t stream_id, c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2) {
-  check_bf16(qkv, "qkv"); check_bf16(ctx, "ctx");
-  TORCH_CHECK(qkv.dim() == 3 && qkv.is_contiguous(), "qkv: contiguous [B,S,3H]");
-  const int B = (int)qkv.size(0), S = (int)qkv.size(1), H = (int)qkv.size(2) / 3;
-  c10::cuda::CUDAGuard guard(qkv.device());
-  b200::attention_fwd(qkv.data_ptr(), seqlens.data_ptr<int>(), ctx.data_ptr(), lse.data_ptr<float>(), B, S, (int)heads,
-                      H / (int)heads, (float)scale, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
-                      mk_fp8(q8, meta8, e5m2, ctx.numel()), cur_stream());
+// The attention kernels need head_dim 64 and S <= 512 with S % 8 == 0.  Padded form: qkv [B, S, 3H] with per-sequence
+// valid lengths `seqlens` (int32 [B]).  Varlen form (`cu_seqlens` given): qkv packed [T, 3H], sequence b is rows
+// cu_seqlens[b] .. cu_seqlens[b + 1] (int32 [B + 1], B = lse.size(0)), S the padded length that sizes lse [B, h, S];
+// it writes no fp8 side output.  Everything is checked before anything is launched.
+struct AttnShape {
+  int B, S, H;
+  long long rows;                  // token rows of qkv: B * S, or T
+  const int* seqlens;              // seqlens (padded) or nullptr
+  const int* cu;                   // cu_seqlens (varlen) or nullptr
+};
+AttnShape check_attention(const Tensor& qkv, const c10::optional<Tensor>& seqlens, const Tensor& lse, int64_t heads,
+                          const c10::optional<Tensor>& cu_seqlens, int64_t S_arg, bool fp8) {
+  const bool varlen = cu_seqlens.has_value() && cu_seqlens->defined();
+  TORCH_CHECK(qkv.dim() == (varlen ? 2 : 3) && qkv.is_contiguous(),
+              varlen ? "attention: qkv must be a contiguous packed [T, 3H] tensor" : "attention: qkv must be a contiguous [B, S, 3H] tensor");
+  AttnShape a;
+  a.H = (int)(qkv.size(-1) / 3);
+  TORCH_CHECK(heads > 0 && qkv.size(-1) % 3 == 0 && a.H % heads == 0 && a.H / heads == 64,
+              "attention: the kernels need head dim 64 (got hidden ", a.H, " over ", heads, " heads)");
+  const int64_t S = varlen ? S_arg : qkv.size(1);
+  TORCH_CHECK(S <= 512 && S % 8 == 0, "attention: the kernels need S <= 512 and S % 8 == 0 (got S = ", S, ")");
+  a.S = (int)S;
+  if (varlen) {
+    TORCH_CHECK(!fp8, "attention: the varlen form writes no fp8 side output");
+    TORCH_CHECK(lse.dim() == 3 && lse.size(1) == heads && lse.size(2) == S, "attention: lse must be [B, heads, S]");
+    a.B = (int)lse.size(0);
+    const Tensor& cu = *cu_seqlens;
+    TORCH_CHECK(cu.scalar_type() == at::kInt && cu.is_contiguous() && cu.dim() == 1 && cu.numel() == a.B + 1,
+                "attention: cu_seqlens must be a contiguous int32 tensor of B + 1 = ", a.B + 1, " entries");
+    TORCH_CHECK(cu.device() == qkv.device(), "attention: cu_seqlens must be on the device of qkv");
+    a.rows = qkv.size(0);
+    a.seqlens = nullptr;
+    a.cu = cu.data_ptr<int>();
+  } else {
+    TORCH_CHECK(seqlens.has_value() && seqlens->defined(), "attention: the padded form needs seqlens");
+    a.B = (int)qkv.size(0);
+    a.rows = (long long)a.B * a.S;
+    a.seqlens = seqlens->data_ptr<int>();
+    a.cu = nullptr;
+  }
+  return a;
 }
-void attention_bwd(Tensor qkv, Tensor seqlens, Tensor ctx, Tensor dctx, Tensor lse, Tensor dqkv, Tensor delta_ws,
-                   c10::optional<Tensor> dq_acc, int64_t heads, double scale, double p_drop, int64_t seed, int64_t stream_id,
-                   c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2) {
+
+void attention_fwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor lse, int64_t heads, double scale,
+                   double p_drop, int64_t seed, int64_t stream_id, c10::optional<Tensor> q8, c10::optional<Tensor> meta8,
+                   bool e5m2, c10::optional<Tensor> cu_seqlens, int64_t S) {
+  const AttnShape a = check_attention(qkv, seqlens, lse, heads, cu_seqlens, S, q8.has_value() && q8->defined());
+  check_bf16(qkv, "qkv"); check_bf16(ctx, "ctx");
+  TORCH_CHECK(ctx.numel() == a.rows * a.H && ctx.is_contiguous(), "attention_fwd: ctx must be contiguous [rows, H]");
+  c10::cuda::CUDAGuard guard(qkv.device());
+  b200::attention_fwd(qkv.data_ptr(), a.seqlens, ctx.data_ptr(), lse.data_ptr<float>(), a.B, a.S, (int)heads,
+                      a.H / (int)heads, (float)scale, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
+                      mk_fp8(q8, meta8, e5m2, ctx.numel()), cur_stream(), a.cu, a.rows);
+}
+void attention_bwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor dctx, Tensor lse, Tensor dqkv,
+                   Tensor delta_ws, c10::optional<Tensor> dq_acc, int64_t heads, double scale, double p_drop, int64_t seed,
+                   int64_t stream_id, c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2,
+                   c10::optional<Tensor> cu_seqlens, int64_t S) {
+  const AttnShape a = check_attention(qkv, seqlens, lse, heads, cu_seqlens, S, q8.has_value() && q8->defined());
   check_bf16(qkv, "qkv"); check_bf16(ctx, "ctx"); check_bf16(dctx, "dctx"); check_bf16(dqkv, "dqkv");
   TORCH_CHECK(qkv.is_contiguous() && ctx.is_contiguous() && dctx.is_contiguous() && dqkv.is_contiguous(), "attention_bwd needs contiguous tensors");
-  const int B = (int)qkv.size(0), S = (int)qkv.size(1), H = (int)qkv.size(2) / 3;
+  TORCH_CHECK(ctx.numel() == a.rows * a.H && dctx.numel() == ctx.numel() && dqkv.numel() == qkv.numel(),
+              "attention_bwd: ctx / dctx [rows, H] and dqkv like qkv");
+  TORCH_CHECK(!dq_acc.has_value() || !dq_acc->defined() || dq_acc->numel() >= a.rows * a.H,
+              "attention_bwd: dq_acc must hold [rows, H] floats");
   c10::cuda::CUDAGuard guard(qkv.device());
-  b200::attention_bwd(qkv.data_ptr(), seqlens.data_ptr<int>(), ctx.data_ptr(), dctx.data_ptr(), lse.data_ptr<float>(),
-                      dqkv.data_ptr(), delta_ws.data_ptr<float>(), opt_f32(dq_acc), B, S, (int)heads, H / (int)heads, (float)scale,
-                      mk_seed(seed), (unsigned)stream_id, (float)p_drop, mk_fp8(q8, meta8, e5m2, dqkv.numel()), cur_stream());
+  b200::attention_bwd(qkv.data_ptr(), a.seqlens, ctx.data_ptr(), dctx.data_ptr(), lse.data_ptr<float>(),
+                      dqkv.data_ptr(), delta_ws.data_ptr<float>(), opt_f32(dq_acc), a.B, a.S, (int)heads, a.H / (int)heads,
+                      (float)scale, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
+                      mk_fp8(q8, meta8, e5m2, dqkv.numel()), cur_stream(), a.cu, a.rows);
 }
 
 void fused_allreduce_lamb(int64_t rank, int64_t world, bool use_multicast, std::vector<int64_t> grad_ptrs,

@@ -22,9 +22,11 @@ void dropout_mask(void* out, long long n_elems, Seed seed, unsigned int stream, 
 void colsum_bf16(const void* x, int M, int N, int ld, float* out, cudaStream_t st);
 void embedding_fwd(const int* ids, const int* seg, const void* word, const void* pos, const void* type,
                    const float* gamma, const float* beta, void* e_out, void* y, float* mean, float* rstd, int M, int S,
-                   int H, float eps, Seed seed, unsigned int stream, float p_drop, cudaStream_t st);
+                   int H, float eps, Seed seed, unsigned int stream, float p_drop, cudaStream_t st,
+                   const int* pos_ids = nullptr);
+// pos_ids (int32 [M], optional): position row of every token row; without it the position is row % S
 void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float* gword, float* gpos, float* gtype,
-                           int M, int S, int H, int type_rows, cudaStream_t st);
+                           int M, int S, int H, int type_rows, cudaStream_t st, const int* pos_ids = nullptr);
 void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st);
 void gather_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st);
 void scatter_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st);
@@ -52,11 +54,16 @@ void arena_adam(float* g, float* p, float* m, float* v, void* shadow, const int*
                 float weight_decay, int step, int bias_correction, int adam_w_mode, cudaStream_t st);
 
 // attention_sm90.cu
+// Padded form (cu_seqlens == nullptr): qkv [B*S, 3H], the valid keys of sequence b are a prefix of length seqlens[b].
+// Varlen form: qkv [T, 3H] packed, sequence b is rows cu_seqlens[b] .. cu_seqlens[b + 1] (int32 [B + 1]); S is the
+// padded length (grid, lse / delta [B, h, S], dropout counter stride) and seqlens is unused.  No fp8 side outputs.
 void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, int B, int S, int h, int d,
-                   float scale, Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st);
+                   float scale, Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
+                   const int* cu_seqlens = nullptr, long long T = 0);
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
-                   Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st);
+                   Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
+                   const int* cu_seqlens = nullptr, long long T = 0);
 
 // comm.cu -- fused peer-memory all-reduce + partitioned LAMB (one cooperative kernel per step)
 struct FusedLambLaunch {

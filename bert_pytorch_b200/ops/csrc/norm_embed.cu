@@ -527,16 +527,17 @@ dgelu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __re
 }
 
 // ------------------------------------------------------------------------------------------------
-// Embedding forward: e = word[id] + pos[s] (+ type[seg]); y = dropout(LN(e)); saves e, mean, rstd
+// Embedding forward: e = word[id] + pos[s] (+ type[seg]); y = dropout(LN(e)); saves e, mean, rstd.
+// s = row % S for a padded [B, S] batch; POS_IDS: s = pos_ids[row] (packed rows of an unpadded batch).
 // ------------------------------------------------------------------------------------------------
-template <int CHUNKS>
+template <int CHUNKS, bool POS_IDS = false>
 __global__ void __launch_bounds__(LN_WARPS * 32)
 embed_fwd_kernel(const int* __restrict__ ids, const int* __restrict__ seg, const __nv_bfloat16* __restrict__ word,
                  const __nv_bfloat16* __restrict__ pos, const __nv_bfloat16* __restrict__ type,
                  const float* __restrict__ gamma, const float* __restrict__ beta, __nv_bfloat16* __restrict__ e_out,
                  __nv_bfloat16* __restrict__ y, float* __restrict__ mean_out, float* __restrict__ rstd_out, int M,
                  int S, int H, float eps, Seed seed_in, unsigned int stream, unsigned int thresh16,
-                 float drop_scale) {
+                 float drop_scale, const int* __restrict__ pos_ids) {
   const unsigned long long seed = seed_in.value();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float g[CHUNKS][8], b[CHUNKS][8];
@@ -545,7 +546,7 @@ embed_fwd_kernel(const int* __restrict__ ids, const int* __restrict__ seg, const
   for (int row = blockIdx.x * LN_WARPS + warp; row < M; row += gridDim.x * LN_WARPS) {
     float v[CHUNKS][8], t0[CHUNKS][8];
     load_row<CHUNKS>(word + (size_t)ids[row] * H, H, lane, v);
-    load_row<CHUNKS>(pos + (size_t)(row % S) * H, H, lane, t0);
+    load_row<CHUNKS>(pos + (size_t)(POS_IDS ? pos_ids[row] : row % S) * H, H, lane, t0);
 #pragma unroll
     for (int c = 0; c < CHUNKS; ++c)
 #pragma unroll
@@ -585,11 +586,12 @@ embed_fwd_kernel(const int* __restrict__ ids, const int* __restrict__ seg, const
   }
 }
 
-// Embedding backward scatter: de [M,H] (bf16) is added into the fp32 gradient tables.
+// Embedding backward scatter: de [M,H] (bf16) is added into the fp32 gradient tables (position row: pos_ids[row] when
+// given, else row % S).
 __global__ void __launch_bounds__(256)
 embed_bwd_scatter_kernel(const __nv_bfloat16* __restrict__ de, const int* __restrict__ ids,
                          const int* __restrict__ seg, float* __restrict__ gword, float* __restrict__ gpos,
-                         float* __restrict__ gtype, int M, int S, int H) {
+                         float* __restrict__ gtype, int M, int S, int H, const int* __restrict__ pos_ids) {
   const int per_row = H / 8;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)M * per_row;
        i += (size_t)gridDim.x * blockDim.x) {
@@ -603,7 +605,8 @@ embed_bwd_scatter_kernel(const __nv_bfloat16* __restrict__ de, const int* __rest
       f[2 * t] = p.x;
       f[2 * t + 1] = p.y;
     }
-    float* dst[3] = {gword + (size_t)ids[row] * H + col, gpos ? gpos + (size_t)(row % S) * H + col : nullptr,
+    float* dst[3] = {gword + (size_t)ids[row] * H + col,
+                     gpos ? gpos + (size_t)(pos_ids ? pos_ids[row] : row % S) * H + col : nullptr,
                      gtype ? gtype + (size_t)seg[row] * H + col : nullptr};
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -850,27 +853,36 @@ void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int
 
 void embedding_fwd(const int* ids, const int* seg, const void* word, const void* pos, const void* type,
                    const float* gamma, const float* beta, void* e_out, void* y, float* mean, float* rstd, int M, int S,
-                   int H, float eps, Seed seed, unsigned int stream, float p_drop, cudaStream_t st) {
+                   int H, float eps, Seed seed, unsigned int stream, float p_drop, cudaStream_t st, const int* pos_ids) {
   unsigned int th; float sc;
   drop_params(p_drop, th, sc);
-  DISPATCH_CHUNKS(H, (embed_fwd_kernel<CH><<<ln_grid(M), LN_WARPS * 32, 0, st>>>(
-      ids, seg, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type, gamma, beta,
-      (__nv_bfloat16*)e_out, (__nv_bfloat16*)y, mean, rstd, M, S, H, eps, seed, stream, th, sc)));
+  if (pos_ids != nullptr)
+    DISPATCH_CHUNKS(H, (embed_fwd_kernel<CH, true><<<ln_grid(M), LN_WARPS * 32, 0, st>>>(
+        ids, seg, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type, gamma, beta,
+        (__nv_bfloat16*)e_out, (__nv_bfloat16*)y, mean, rstd, M, S, H, eps, seed, stream, th, sc, pos_ids)));
+  else
+    DISPATCH_CHUNKS(H, (embed_fwd_kernel<CH><<<ln_grid(M), LN_WARPS * 32, 0, st>>>(
+        ids, seg, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type, gamma, beta,
+        (__nv_bfloat16*)e_out, (__nv_bfloat16*)y, mean, rstd, M, S, H, eps, seed, stream, th, sc, nullptr)));
 }
 
 void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float* gword, float* gpos, float* gtype,
-                           int M, int S, int H, int type_rows, cudaStream_t st) {
+                           int M, int S, int H, int type_rows, cudaStream_t st, const int* pos_ids) {
   const size_t work = (size_t)M * (H / 8);
   int grid = (int)((work + 255) / 256);
   if (grid > num_sms() * 16) grid = num_sms() * 16;
-  if (M % S == 0 && H % 8 == 0 && (gtype == nullptr || type_rows == 2)) {
+  if (pos_ids == nullptr && M % S == 0 && H % 8 == 0 && (gtype == nullptr || type_rows == 2)) {
     // word rows: scatter with atomics (30 k rows, little contention); position / token-type rows: reductions
-    embed_bwd_scatter_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)de, ids, seg, gword, nullptr, nullptr, M, S, H);
+    embed_bwd_scatter_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)de, ids, seg, gword, nullptr, nullptr, M, S, H,
+                                                   nullptr);
     dim3 g2((H + 255) / 256, (S + 7) / 8);
     embed_bwd_postype_kernel<<<g2, 256, 0, st>>>((const __nv_bfloat16*)de, seg, gpos, gtype, M / S, S, H);
     return;
   }
-  embed_bwd_scatter_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)de, ids, seg, gword, gpos, gtype, M, S, H);
+  // packed rows (pos_ids) or a ragged batch: every table row by atomics
+  if (grid > 0)
+    embed_bwd_scatter_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)de, ids, seg, gword, gpos, gtype, M, S, H,
+                                                   pos_ids);
 }
 
 void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st) {
