@@ -443,6 +443,16 @@ def _uniform(optimizer, key):
     return optimizer.param_groups[0][key]
 
 
+def _uniform_decay(optimizer) -> float:
+    """The weight decay of the decaying slots.  The fused kernels take one value and a per-slot decay flag (set by
+    ``ParamArena.bind_optimizer`` from ``weight_decay != 0``), so the groups may mix 0 with one non-zero value only."""
+    wds = {float(g["weight_decay"]) for g in optimizer.param_groups} - {0.0}
+    if len(wds) > 1:
+        raise NotImplementedError(f"fused arena optimizer needs one non-zero 'weight_decay' across the param groups, "
+                                  f"got {sorted(wds)}")
+    return wds.pop() if wds else 0.0
+
+
 def arena_lamb_step(arena, optimizer, inv_scale=None, found_inf=None) -> None:
     """One LAMB step over the arena (3 launches + 2 memsets).  Weight decay is per slot (decay flag x
     the single non-zero group value), every other hyper-parameter must agree across groups -- which is
@@ -451,10 +461,7 @@ def arena_lamb_step(arena, optimizer, inv_scale=None, found_inf=None) -> None:
     lr = _uniform(optimizer, "lr")
     b1, b2 = _uniform(optimizer, "betas")
     eps = _uniform(optimizer, "eps")
-    wds = sorted({float(g["weight_decay"]) for g in optimizer.param_groups})
-    wd = max(wds)
-    for g in optimizer.param_groups:      # decay flag of a slot must agree with its group's decay
-        pass
+    wd = _uniform_decay(optimizer)
     step = int(optimizer.param_groups[0].get("step", 0)) + 1
     ext = extension()
     inv = inv_scale.reshape(1) if inv_scale is not None else None
@@ -480,10 +487,15 @@ def arena_adam_step(arena, optimizer, inv_scale=None, found_inf=None) -> None:
     lr = _uniform(optimizer, "lr")
     b1, b2 = _uniform(optimizer, "betas")
     eps = _uniform(optimizer, "eps")
-    wd = max(float(g["weight_decay"]) for g in optimizer.param_groups)
+    wd = _uniform_decay(optimizer)
     step = int(optimizer.param_groups[0].get("step", 0)) + 1
     inv = inv_scale.reshape(1) if inv_scale is not None else None
     fi = found_inf.reshape(1) if found_inf is not None else None
+    if inv is not None and fi is not None:
+        # the Adam kernel only reads found_inf (LAMB's norm pass sets it): unscale and check the gradients first
+        extension().flat_unscale(arena.flat_grad, inv, fi)
+        _count()
+        inv = None
     extension().arena_adam(arena.flat_grad, arena.flat_param, arena.exp_avg, arena.exp_avg_sq, arena.flat_shadow,
                            T["ct"], T["cs"], T["cl"], T["decay"], inv, fi, float(lr), float(b1), float(b2), float(eps),
                            float(wd), step, bool(_uniform(optimizer, "bias_correction")), bool(optimizer.adam_w_mode))

@@ -346,6 +346,7 @@ void flat_sumsq(Tensor g, c10::optional<Tensor> inv_scale, Tensor stats, c10::op
 }
 void flat_unscale(Tensor g, Tensor inv_scale, Tensor found_inf) {
   c10::cuda::CUDAGuard guard(g.device());
+  TORCH_CHECK(g.numel() % 4 == 0, "arena size must be a multiple of 4");
   b200::flat_unscale(g.data_ptr<float>(), g.numel(), inv_scale.data_ptr<float>(), found_inf.data_ptr<float>(), cur_stream());
 }
 void arena_lamb(Tensor g, Tensor p, Tensor m, Tensor v, c10::optional<Tensor> shadow, Tensor chunk_tensor,

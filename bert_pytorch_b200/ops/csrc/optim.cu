@@ -126,7 +126,8 @@ flat_unscale_kernel(float* __restrict__ g, long long n, const float* __restrict_
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     float4 v = g4[i];
     v.x *= is; v.y *= is; v.z *= is; v.w *= is;
-    bad |= !isfinite(v.x + v.y + v.z + v.w);
+    // per element: the sum of four finite values can overflow (3e38 + 3e38) and would flag a clean step
+    bad |= !(isfinite(v.x) && isfinite(v.y) && isfinite(v.z) && isfinite(v.w));
     g4[i] = v;
   }
   if (bad) *found_inf = 1.f;

@@ -153,7 +153,7 @@ class PeerComm(TorchComm):
         """reduce-scatter + unscale + partitioned LAMB + all-gather, one kernel.  ``optimizer`` supplies the
         hyper-parameters and owns the (arena backed) moment buffers."""
         from .. import ops
-        from ..ops.api import _uniform
+        from ..ops.api import _uniform, _uniform_decay
         A = self.arena
         if A is None or A.exp_avg is None:
             raise RuntimeError("PeerComm.adopt(arena) and arena.bind_optimizer(optimizer) must be called first")
@@ -163,7 +163,7 @@ class PeerComm(TorchComm):
             self._decay = decay
         lr = _uniform(optimizer, "lr")
         b1, b2 = _uniform(optimizer, "betas")
-        wd = max(float(g["weight_decay"]) for g in optimizer.param_groups)
+        wd = _uniform_decay(optimizer)
         step = int(optimizer.param_groups[0].get("step", 0)) + 1
         self.epoch += 1
         mc = self.use_multicast

@@ -175,6 +175,21 @@ def test_adam_and_bertadam():
         BertAdam([q], lr=-1.0)
 
 
+def test_fused_optimizers_take_one_non_zero_weight_decay():
+    """The fused arena kernels apply one weight decay to every decaying slot: the groups may mix 0 with a single
+    non-zero value, and anything else is refused rather than applied as the largest value."""
+    from types import SimpleNamespace
+    from bert_pytorch_b200.ops.api import _uniform_decay
+    opt = lambda *wds: SimpleNamespace(param_groups=[{"weight_decay": w} for w in wds])
+    assert _uniform_decay(opt(0.01, 0.0)) == 0.01
+    assert _uniform_decay(opt(0.0, 0.01, 0.01)) == 0.01
+    assert _uniform_decay(opt(0.0, 0.0)) == 0.0
+    assert _uniform_decay(opt(0.01)) == 0.01
+    for wds in ((0.01, 0.001), (0.01, 0.0, 0.001), (0.01, -0.01)):
+        with pytest.raises(NotImplementedError, match="weight_decay"):
+            _uniform_decay(opt(*wds))
+
+
 def test_grad_scaler_dynamics_and_state_dict():
     p = torch.nn.Parameter(torch.ones(4))
     opt = Lamb([p], lr=0.1)
