@@ -4,7 +4,9 @@
 //   every GEMM operand site owns a 4-float record  meta = {amax, scale, inv_scale, _}  on the device
 //   quantise:     q = sat_fp8(x * scale)      and   amax = max(amax, |x|)      (one pass over x, 3 B/element)
 //   GEMM:         D = (qa . qb) * inv_scale_a * inv_scale_b                     (read by the epilogue from meta)
-//   end of step:  scale = fmax / amax (power of two, so re-scaling is exact), inv_scale = 1 / scale, amax = 0
+//   end of step:  scale = 2^e with e the largest integer such that amax * margin * 2^e <= fmax, clamped to
+//                 [-126, 126] (power of two, so re-scaling is exact; scale and inv_scale = 1 / scale are both finite,
+//                 normal floats for any amax), then amax = 0.  amax = 0 or non-finite keeps the old scale.
 // Nothing syncs with the host; the first step after enabling fp8 calibrates with fp8_amax + fp8_update.
 #include <cuda_fp8.h>
 
@@ -68,18 +70,22 @@ __global__ void __launch_bounds__(256) fp8_amax_kernel(const __nv_bfloat16* __re
   if ((threadIdx.x & 31) == 0 && amax > 0.f) atomic_max_nonneg(meta, isfinite(amax) ? amax : 3.0e38f);
 }
 
-// one thread per record; fmax_e5m2_mask bit i set -> record i quantises to e5m2 (max 57344) else e4m3 (448)
+// one thread per record; is_e5m2[i] != 0 -> record i quantises to e5m2 (max 57344) else e4m3 (448)
 __global__ void fp8_update_kernel(float* __restrict__ meta, int nrec, const int* __restrict__ is_e5m2, float margin_pow2) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nrec) return;
   float* m = meta + 4 * i;
   const float amax = m[0];
   if (amax > 0.f && isfinite(amax)) {
-    const float fmax = is_e5m2[i] ? 57344.f : 448.f;
-    // largest power of two with amax * scale <= fmax / margin
-    const float s = exp2f(floorf(log2f(fmax / (amax * margin_pow2))));
-    m[1] = s;
-    m[2] = 1.f / s;
+    // largest e with amax * margin * 2^e <= fmax, from exact mantissas and exponents: fmax / (amax * margin) in fp32
+    // overflows for a tiny amax (< 1.3e-36 for e4m3) and amax * margin for one near FLT_MAX
+    int e_x, e_f;
+    const double m_x = frexp((double)amax * (double)margin_pow2, &e_x);   // exact: a 48-bit product
+    const double m_f = frexp(is_e5m2[i] ? 57344.0 : 448.0, &e_f);
+    int e = e_f - e_x - (m_x > m_f ? 1 : 0);
+    e = min(126, max(-126, e));                      // scale and inv_scale both finite, normal powers of two
+    m[1] = ldexpf(1.f, e);
+    m[2] = ldexpf(1.f, -e);
   }
   m[0] = 0.f;
 }
