@@ -545,7 +545,9 @@ class FusedEncoderEngine:
         d = H // h
         t = qkv.view(B, S, 3, h, d)
         q, k, v = (t[:, :, i].transpose(1, 2) for i in range(3))
-        mask = (torch.arange(S, device=qkv.device)[None, :] < seqlens[:, None])[:, None, None, :]
+        # the kernels' rule: an all-zero mask row (length 0) attends to every key
+        n = torch.where(seqlens > 0, seqlens, S)
+        mask = (torch.arange(S, device=qkv.device)[None, :] < n[:, None])[:, None, None, :]
         if training:
             with torch.enable_grad():
                 q, k, v = (z.detach().requires_grad_(True) for z in (q, k, v))

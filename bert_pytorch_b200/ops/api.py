@@ -314,7 +314,8 @@ def _attn_shape(qkv: torch.Tensor, seqlens, cu_seqlens, S):
 
 def attention_fwd(qkv: torch.Tensor, seqlens: Optional[torch.Tensor], heads: int, *, p_drop=0.0, seed=0, stream=0,
                   fp8=None, cu_seqlens: Optional[torch.Tensor] = None, S: Optional[int] = None):
-    """Padded form: qkv [B, S, 3H], valid keys of sequence b = its first ``seqlens[b]`` -> ctx [B, S, H].
+    """Padded form: qkv [B, S, 3H], valid keys of sequence b = its first ``seqlens[b]`` (clamped to S; 0, an all-zero
+    mask row, means all S keys, as under the model's additive mask) -> ctx [B, S, H].
     Varlen form (``cu_seqlens``, ``S``, ``seqlens=None``): qkv packed [T, 3H], sequence b = rows cu_seqlens[b] ..
     cu_seqlens[b + 1] -> ctx [T, H]; ``S`` is the padded length (at most 512, a multiple of 8), which sizes the grid
     and lse, and strides the dropout counter, so the keep decisions are the padded call's.  lse is [B, heads, S] in

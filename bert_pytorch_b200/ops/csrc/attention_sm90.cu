@@ -1,5 +1,7 @@
 // Fused multi-head attention for BERT (non-causal, key-padding mask given as per-sequence valid length,
 // head_dim 64, S <= 512) on wgmma (sm_90a): scores, softmax, dropout and P V never leave the SM.
+// Padded form: the valid keys of sequence b are its first min(seqlens[b], S); seqlens[b] <= 0 (an all-zero mask row)
+// makes all S keys valid, which is what the model's additive -10000 mask computes, so every output stays finite.
 //
 // Data layout: qkv is the QKV-GEMM output [B*S, 3H] (token-major, q|k|v, head-major inside), so the Q / K / V tiles
 // of a head are 64-column TMA boxes of that matrix; ctx / dctx are [B*S, H].
@@ -139,6 +141,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     if (qb * QT >= seqlen) return;                      // CTA uniform, before any mbarrier or TMA work
   } else {
     seqlen = min(p.seqlens[b], p.S);
+    if (seqlen <= 0) seqlen = p.S;                      // a fully masked sequence attends to every key
     row0 = b * p.S;
   }
   const int nkb = max(1, (seqlen + KT - 1) / KT);       // key blocks that contain valid keys
@@ -338,6 +341,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     if (kb * KT >= seqlen) return;                      // CTA uniform, before any mbarrier or TMA work
   } else {
     seqlen = min(p.seqlens[b], p.S);
+    if (seqlen <= 0) seqlen = p.S;                      // a fully masked sequence attends to every key
     row0 = b * p.S;
   }
   const int q_end = VARLEN ? seqlen : p.S;              // query rows (and rows of dK / dV) that exist

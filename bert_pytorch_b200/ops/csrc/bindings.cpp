@@ -376,7 +376,8 @@ void arena_adam(Tensor g, Tensor p, Tensor m, Tensor v, c10::optional<Tensor> sh
 }
 
 // The attention kernels need head_dim 64 and S <= 512 with S % 8 == 0.  Padded form: qkv [B, S, 3H] with per-sequence
-// valid lengths `seqlens` (int32 [B]).  Varlen form (`cu_seqlens` given): qkv packed [T, 3H], sequence b is rows
+// valid lengths `seqlens` (int32 [B]), clamped to S; a length <= 0 (an all-zero mask row) attends to all S keys, as the
+// model's additive mask does.  Varlen form (`cu_seqlens` given): qkv packed [T, 3H], sequence b is rows
 // cu_seqlens[b] .. cu_seqlens[b + 1] (int32 [B + 1], B = lse.size(0)), S the padded length that sizes lse [B, h, S];
 // it writes no fp8 side output.  Everything is checked before anything is launched.
 struct AttnShape {

@@ -54,7 +54,8 @@ void arena_adam(float* g, float* p, float* m, float* v, void* shadow, const int*
                 float weight_decay, int step, int bias_correction, int adam_w_mode, cudaStream_t st);
 
 // attention_sm90.cu
-// Padded form (cu_seqlens == nullptr): qkv [B*S, 3H], the valid keys of sequence b are a prefix of length seqlens[b].
+// Padded form (cu_seqlens == nullptr): qkv [B*S, 3H], the valid keys of sequence b are a prefix of length seqlens[b]
+// (clamped to S; a length <= 0 means all S keys).
 // Varlen form: qkv [T, 3H] packed, sequence b is rows cu_seqlens[b] .. cu_seqlens[b + 1] (int32 [B + 1]); S is the
 // padded length (grid, lse / delta [B, h, S], dropout counter stride) and seqlens is unused.  No fp8 side outputs.
 void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, int B, int S, int h, int d,

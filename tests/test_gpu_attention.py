@@ -1,6 +1,5 @@
-"""wgmma fused attention (forward + backward) vs an fp32 PyTorch reference of the same op."""
-import math
-
+"""wgmma fused attention (forward + backward): run-to-run agreement under dropout, which exposes races.  The accuracy
+tests against an fp64 reference are in test_gpu_attention_reference.py."""
 import pytest
 import torch
 
@@ -12,78 +11,6 @@ def _api():
     from bert_pytorch_b200.ops import api
     assert ops.available()
     return api
-
-
-def _ref(qkv, seqlens, heads):
-    B, S, H3 = qkv.shape
-    H = H3 // 3
-    d = H // heads
-    t = qkv.float().view(B, S, 3, heads, d)
-    q, k, v = (t[:, :, i].transpose(1, 2) for i in range(3))
-    scores = q @ k.transpose(-1, -2) / math.sqrt(d)
-    mask = torch.arange(S, device=qkv.device)[None, :] < seqlens[:, None]
-    scores = scores.masked_fill(~mask[:, None, None, :], float("-inf"))
-    p = torch.softmax(scores, dim=-1)
-    lse = torch.logsumexp(scores, dim=-1)
-    return (p @ v).transpose(1, 2).reshape(B, S, H), lse
-
-
-@pytest.mark.parametrize("B,S,heads,lens", [
-    (2, 128, 2, [128, 77]), (3, 128, 4, [128, 1, 64]), (2, 256, 2, [256, 130]), (2, 512, 2, [512, 300]),
-    (2, 384, 2, [384, 129]), (1, 64, 2, [50]),
-])
-def test_attention_fwd_bwd_no_dropout(B, S, heads, lens):
-    K = _api()
-    torch.manual_seed(0)
-    H = heads * 64
-    qkv = (torch.randn(B, S, 3 * H, device="cuda") * 0.7).to(torch.bfloat16)
-    seqlens = torch.tensor(lens, device="cuda", dtype=torch.int32)
-    ctx, lse = K.attention_fwd(qkv, seqlens, heads)
-    leaf = qkv.float().requires_grad_(True)
-    ref, ref_lse = _ref(leaf, seqlens, heads)
-    err = (ctx.float() - ref).abs().max().item()
-    assert err < 2e-2, err
-    assert (lse - ref_lse).abs().max().item() < 2e-2
-    dctx = (torch.randn(B, S, H, device="cuda") * 0.5).to(torch.bfloat16)
-    ref.backward(dctx.float())
-    dqkv = K.attention_bwd(qkv, seqlens, ctx, dctx, lse, heads)
-    g = leaf.grad
-    scale = g.abs().max().item()
-    # padded *keys* get exactly zero dK/dV in both; compare everything
-    err = (dqkv.float() - g).abs().max().item()
-    assert err < 4e-2 * max(scale, 1.0), (err, scale)
-
-
-@pytest.mark.parametrize("S", [256, 128])          # 128: one key block
-def test_attention_dropout_statistics_and_adjoint(S):
-    K = _api()
-    torch.manual_seed(0)
-    B, heads = 2, 2
-    H = heads * 64
-    qkv = (torch.randn(B, S, 3 * H, device="cuda") * 0.5).to(torch.bfloat16)
-    seqlens = torch.tensor([S, S - 56], device="cuda", dtype=torch.int32)
-    base, _ = K.attention_fwd(qkv, seqlens, heads)
-    outs = [K.attention_fwd(qkv, seqlens, heads, p_drop=0.1, seed=1000 + i, stream=3)[0].float() for i in range(24)]
-    again = K.attention_fwd(qkv, seqlens, heads, p_drop=0.1, seed=1000, stream=3)[0].float()
-    assert torch.equal(outs[0], again)                       # deterministic in (seed, stream)
-    assert not torch.equal(outs[0], outs[1])
-    mean = torch.stack(outs).mean(0)
-    assert (mean - base.float()).abs().mean().item() < 2e-2   # unbiased
-    # adjoint identity in V for a fixed mask: <dO, O(V)> == <dV, V>  (O is linear in V)
-    ctx, lse = K.attention_fwd(qkv, seqlens, heads, p_drop=0.1, seed=7, stream=3)
-    # dO correlated with O so that <dO, O> is a large positive number: a 1 / keep_prob slip between the forward and the
-    # backward mask scaling (11 %) cannot hide behind cancellation
-    dctx = (ctx.float() * 4.0 + 0.25 * torch.randn(B, S, H, device="cuda")).to(torch.bfloat16)
-    dqkv = K.attention_bwd(qkv, seqlens, ctx, dctx, lse, heads, p_drop=0.1, seed=7, stream=3)
-    lhs = (dctx.float() * ctx.float()).sum().item()
-    v = qkv.float().view(B, S, 3, H)[:, :, 2]
-    dv = dqkv.float().view(B, S, 3, H)[:, :, 2]
-    rhs = (dv * v).sum().item()
-    assert lhs > 50.0 and abs(lhs - rhs) < 2e-2 * abs(lhs), (lhs, rhs)
-    # and with a different seed the identity must break (proves the mask really matters)
-    dqkv2 = K.attention_bwd(qkv, seqlens, ctx, dctx, lse, heads, p_drop=0.1, seed=8, stream=3)
-    rhs2 = (dqkv2.float().view(B, S, 3, H)[:, :, 2] * v).sum().item()
-    assert abs(rhs2 - rhs) > 1e-3 * max(abs(rhs), 1.0)
 
 
 @pytest.mark.parametrize("B,S,heads,lens,p_drop", [
