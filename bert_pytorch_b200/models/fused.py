@@ -31,6 +31,9 @@ Unpadded mode (``BertModel.unpad``, fine-tuning and inference through :meth:`Fus
 unmasked tokens of the [B, S] batch are packed into T rows (:func:`pack_rows`) and every kernel runs on those rows
 only -- embeddings with explicit position ids, GEMMs / LayerNorms / dropout with M = T, variable-length attention
 over ``cu_seqlens``.  The output is scattered back into a zeroed [B*S, H] tensor.
+Pre-training (``FusedPretrainer`` with ``BertModel.unpad``, ``--unpad``) packs on the device instead (:func:`pack_device`,
+no host sync) into a static row count T_cap from :func:`token_bucket`, so that each bucket replays its own CUDA graph;
+the rows past the real tokens are [PAD] tokens in dummy sequences of their own, finite and with zero gradient.
 """
 from __future__ import annotations
 
@@ -91,11 +94,17 @@ class _LayerSaved:
 @dataclass
 class Packing:
     """The unmasked tokens of a [B, S] batch packed back to back (one record per call, shared by every layer)."""
-    rows: torch.Tensor          # int32 [T]: index b * S + s of every unmasked token, in order
+    rows: Optional[torch.Tensor]  # int32 [T]: index b * S + s of every unmasked token, in order (pack_rows only)
     cu_seqlens: torch.Tensor    # int32 [B + 1]: sequence b is packed rows cu_seqlens[b] .. cu_seqlens[b + 1]
     pos_ids: torch.Tensor       # int32 [T]: position s of every packed row
     T: int
     S: int
+    # device packing of pre-training (pack_device): T is the bucket capacity T_cap, cu_seqlens has B + D + 1 entries
+    # (D dummy sequences over the pad tail), and the token ids / segments come packed already
+    ids: Optional[torch.Tensor] = None       # int32 [T]
+    seg: Optional[torch.Tensor] = None       # int32 [T]
+    cls_rows: Optional[torch.Tensor] = None  # int32 [B]: first packed row of every sequence
+    row_map: Optional[torch.Tensor] = None   # int32 [B * S]: packed row of token (b, s), -1 where masked
 
 
 def pack_rows(attention_mask: torch.Tensor) -> Packing:
@@ -107,6 +116,39 @@ def pack_rows(attention_mask: torch.Tensor) -> Packing:
     cu[1:] = torch.cumsum(keep.sum(dim=1, dtype=torch.int32), 0, dtype=torch.int32)
     return Packing(rows=rows.to(torch.int32), cu_seqlens=cu, pos_ids=(rows % S).to(torch.int32),
                    T=rows.numel(), S=S)
+
+
+# ---- unpadded pre-training: static token buckets -------------------------------------------------------------------
+MAX_TOKEN_BUCKETS = 16
+
+
+def token_bucket(T: int, B: int, S: int):
+    """(T_cap, D) of a micro-batch with T packed tokens: the row capacity of its CUDA graph and the number of dummy
+    sequences that cover the pad tail ``T_cap - T``.  The bucket step is ``g = 128 * ceil(B*S / (128 * 16))`` rows: at
+    most 16 buckets (16 graphs per batch shape), each a whole number of 128-row GEMM tiles, and a pad tail below one
+    step (< 1/16 of the batch).  ``T_cap = min(B*S, ceil(T / g) * g)``; ``D = ceil(g / S)`` dummies of at most S rows
+    always cover the tail, since it is shorter than g."""
+    M = B * S
+    if not 1 <= T <= M:
+        raise ValueError(f"token count {T} outside [1, {M}] for a [{B}, {S}] batch")
+    g = 128 * -(-M // (128 * MAX_TOKEN_BUCKETS))
+    return min(M, -(-T // g) * g), -(-g // S)
+
+
+def packed_tokens(mask: torch.Tensor) -> int:
+    """Number of packed rows of a [B, S] attention mask: its unmasked tokens, where a row without any counts S (the
+    padded attention computes such a row with every key valid).  One host read on a device tensor; none on the pinned
+    host batch."""
+    S = mask.size(-1)
+    n = (mask.reshape(-1, S) != 0).sum(dim=1)
+    return int(torch.where(n > 0, n, torch.full_like(n, S)).sum())
+
+
+def pack_device(input_mask, input_ids, segment_ids, T_cap: int, D: int) -> Packing:
+    """:func:`~bert_pytorch_b200.ops.api.pack_tokens` as a :class:`Packing` (no host sync: capturable)."""
+    ids, seg, pos, cu, cls, row_map = K.pack_tokens(input_mask, input_ids, segment_ids, T_cap, D)
+    return Packing(rows=None, cu_seqlens=cu, pos_ids=pos, T=T_cap, S=input_mask.size(1), ids=ids, seg=seg,
+                   cls_rows=cls, row_map=row_map)
 
 
 @dataclass
@@ -338,7 +380,9 @@ class FusedEncoderEngine:
         if self.has_type:
             seg = (token_type_ids if token_type_ids is not None else torch.zeros_like(input_ids)
                    ).reshape(-1).to(torch.int32).contiguous()
-        if pack is not None:
+        if pack is not None and pack.ids is not None:   # packed on the device already (pack_device)
+            ids, seg, seqlens = pack.ids, pack.seg if seg is not None else None, None
+        elif pack is not None:
             ids = ids.index_select(0, pack.rows)
             seg = seg.index_select(0, pack.rows) if seg is not None else None
             seqlens = None
@@ -707,19 +751,45 @@ class FusedPretrainer:
             return False                      # tapped micro-steps keep Python-side state; the library attention path owns its RNG
         return self.arena.device.type == "cuda"
 
+    def _bucket(self, input_mask, tokens: Optional[int]):
+        """(T_cap, D) of this micro-step when it runs unpadded (``BertModel.unpad``), else None.  fp8 operands and the
+        library attention have no unpadded path (warned once), and K-FAC micro-steps that feed the factors run padded
+        so that their statistics are the padded ones.  Without ``tokens`` the count is read back from the device (one
+        host sync)."""
+        if not getattr(self.model.bert, "unpad", False):
+            return None
+        eng = self.engine
+        if eng.fp8 or _use_sdpa():
+            if not getattr(self, "_unpad_warned", False):
+                warnings.warn("BertModel.unpad: fp8 operands and B200_ATTN=sdpa have no unpadded pre-training path; "
+                              "running padded")
+                self._unpad_warned = True
+            return None
+        kf = getattr(self.model.bert, "_kfac", None)
+        if kf is not None and getattr(kf, "capture", True):
+            return None
+        B, S = input_mask.shape
+        return token_bucket(packed_tokens(input_mask) if tokens is None else int(tokens), B, S)
+
     @torch.no_grad()
     def forward_backward(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
-                         grad_scale: float = 1.0) -> torch.Tensor:
+                         grad_scale: float = 1.0, tokens: Optional[int] = None) -> torch.Tensor:
         """One micro-step.  After ``graph_warmup`` eager calls with the same input signature the whole kernel
         program (forward, loss, backward: ~600 launches) is captured once and replayed as ONE CUDA graph; the
-        dropout seed advances through a device-side step counter inside the graph."""
+        dropout seed advances through a device-side step counter inside the graph.
+
+        Unpadded (``BertModel.unpad``): the program packs the batch on the device into the token bucket of ``tokens``
+        (:func:`packed_tokens` of the mask, a host int; counted on the device when omitted) and computes T_cap rows
+        instead of B * S.  The bucket is part of the graph key: one graph per bucket, all in one memory pool."""
+        bucket = self._bucket(input_mask, tokens)
         if not self._graph_ok():
-            return self._program(input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels, grad_scale)
+            return self._program(input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels, grad_scale,
+                                 bucket=bucket)
         args = (input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels)
         key = (tuple(input_ids.shape), self.model.training, next_sentence_labels is not None,
                segment_ids is not None, tuple(str(t.dtype) for t in args if t is not None),
                bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)), self.engine.fp8,
-               bool(self.grad_push), bool(self.engine.wgrad_side))
+               bool(self.grad_push), bool(self.engine.wgrad_side), bucket)
         ent = self._graphs.setdefault(key, {"calls": 0})
         ent["calls"] += 1
         eng = self.engine
@@ -730,7 +800,7 @@ class FusedPretrainer:
                 ent.pop(k)
         if "graph" not in ent:
             if ent["calls"] <= self.graph_warmup or (eng.fp8 and not eng._fp8_calibrated):
-                return self._program(*args, grad_scale)
+                return self._program(*args, grad_scale, bucket=bucket)
             if self._seed_step is None:
                 self._seed_step = torch.zeros(1, dtype=torch.int64, device=self.arena.device)
                 ops.extension().set_seed_step(self._seed_step)
@@ -751,7 +821,7 @@ class FusedPretrainer:
             try:
                 with torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local", **extra):
                     self._seed_step.add_(1)
-                    loss = self._program(*static, grad_scale, seed=eng._seed_base)
+                    loss = self._program(*static, grad_scale, seed=eng._seed_base, bucket=bucket)
             except Exception as e:            # e.g. an allocator / stream condition this build of torch cannot capture
                 import warnings
                 warnings.warn(f"CUDA-graph capture of the micro-step failed ({type(e).__name__}: {e}); "
@@ -759,7 +829,7 @@ class FusedPretrainer:
                 K.KERNEL_LAUNCHES = n0
                 self.use_graphs = False
                 torch.cuda.synchronize()      # nothing of the captured program ran: the accumulated gradients are intact
-                return self._program(*args, grad_scale)
+                return self._program(*args, grad_scale, bucket=bucket)
             ent.update(graph=graph, static=static, loss=loss, launches=K.KERNEL_LAUNCHES - n0, grad_scale=float(grad_scale))
             K.KERNEL_LAUNCHES = n0            # the capture itself ran nothing
         for dst, src in zip(ent["static"], args):
@@ -772,14 +842,18 @@ class FusedPretrainer:
 
     @torch.no_grad()
     def _program(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
-                 grad_scale: float = 1.0, seed: Optional[int] = None) -> torch.Tensor:
+                 grad_scale: float = 1.0, seed: Optional[int] = None, bucket=None) -> torch.Tensor:
+        """The kernel program of one micro-step; ``bucket`` = (T_cap, D) runs it on the packed tokens of the batch
+        (T_cap rows: the real tokens, then a pad tail of inert [PAD] rows in D dummy sequences)."""
         eng, A, H, V = self.engine, self.arena, self.H, self.V
         B, S = input_ids.shape
-        M = B * S
-        seq, sv = eng.forward(input_ids, segment_ids, input_mask, training=True, seed=seed, dropout=self.model.training)
+        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
+        M = pk.T if pk is not None else B * S
+        seq, sv = eng.forward(input_ids, segment_ids, input_mask, training=True, seed=seed, dropout=self.model.training,
+                              pack=pk)
         labels = masked_lm_labels.to(torch.int32).contiguous()
         mp = self._max_pred(labels)
-        idx, tgt, count = K.mlm_compact(labels, mp)
+        idx, tgt, count = K.mlm_compact(labels, mp, row_map=pk.row_map if pk is not None else None)
         loss = torch.zeros(1, dtype=torch.float32, device=seq.device)
 
         # ---- MLM head forward (masked rows only)
@@ -812,10 +886,14 @@ class FusedPretrainer:
         if self.has_nsp and next_sentence_labels is not None:
             pool, nsp = self.model.bert.pooler.dense_act, self.model.cls.seq_relationship
             pw = A.shadow(eng.prefix + "pooler.dense_act.weight")
-            if self._cls_idx is None or self._cls_idx.numel() != B or self._cls_S != S:
-                self._cls_idx = (torch.arange(B, device=seq.device, dtype=torch.int32) * S).contiguous()
-                self._cls_S = S
-            cls_tok = K.gather_rows(seq, self._cls_idx)                                        # [B, H] bf16
+            if pk is not None:
+                cls_idx = pk.cls_rows
+            else:
+                if self._cls_idx is None or self._cls_idx.numel() != B or self._cls_S != S:
+                    self._cls_idx = (torch.arange(B, device=seq.device, dtype=torch.int32) * S).contiguous()
+                    self._cls_S = S
+                cls_idx = self._cls_idx
+            cls_tok = K.gather_rows(seq, cls_idx)                                              # [B, H] bf16
             pooled = K.gemm(cls_tok, pw, epi=K.EPI_BIAS_TANH, bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
             d_z = K.nsp_head_(pooled, A.shadow("cls.seq_relationship.weight"), nsp.bias, next_sentence_labels.long().view(-1),
                               grad_scale, loss, nsp.weight.grad, nsp.bias.grad)
@@ -833,7 +911,10 @@ class FusedPretrainer:
             K.wgrad_accumulate(d_z, cls_tok, pool.weight.grad)
             K.colsum_accumulate(d_z, pool.bias.grad)
             d_cls = K.gemm(d_z, pw, layout=K.NN)
-            d_seq.view(B, S, H)[:, 0] += d_cls
+            if pk is not None:                     # the same bf16 add at the (distinct) first packed rows
+                d_seq.index_add_(0, pk.cls_rows.long(), d_cls)
+            else:
+                d_seq.view(B, S, H)[:, 0] += d_cls
 
         eng.backward(sv, d_seq)
         return loss.squeeze(0) if loss.dim() else loss

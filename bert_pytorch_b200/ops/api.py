@@ -261,14 +261,47 @@ def embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S: int, *, pos_ids: 
     _count()
 
 
-def mlm_compact(labels: torch.Tensor, max_pred: int):
+def mlm_compact(labels: torch.Tensor, max_pred: int, row_map: Optional[torch.Tensor] = None):
+    """``row_map`` (int32 [B * S], from :func:`pack_tokens`): ``idx`` holds packed rows instead of ``b * S + s``, and a
+    label whose token is masked is dropped (not counted)."""
     B = labels.size(0)
     idx = torch.empty(B * max_pred, dtype=torch.int32, device=labels.device)
     tgt = torch.empty_like(idx)
     count = torch.empty(1, dtype=torch.int32, device=labels.device)
-    extension().mlm_compact(labels, max_pred, idx, tgt, count)
+    if row_map is None:
+        extension().mlm_compact(labels, max_pred, idx, tgt, count)
+    else:
+        extension().mlm_compact(labels, max_pred, idx, tgt, count, row_map)
     _count()
     return idx, tgt, count
+
+
+def pack_tokens(input_mask: torch.Tensor, input_ids: torch.Tensor, segment_ids: Optional[torch.Tensor], T_cap: int,
+                D: int):
+    """Packs the unmasked tokens of a [B, S] batch into ``T_cap`` rows on the device, with no host sync (it runs inside
+    a captured graph).  Returns int32 ``(ids, seg, pos_ids, cu_seqlens, cls_rows, row_map)``:
+
+    * ``ids``, ``seg``, ``pos_ids`` [T_cap]: token id, segment and position of every unmasked token in ``b * S + s``
+      order, then the pad tail (id 0, segment 0, position inside its dummy sequence);
+    * ``cu_seqlens`` [B + D + 1]: the B sequences, then D dummy sequences of at most S rows over the pad tail;
+    * ``cls_rows`` [B]: first packed row of every sequence; ``row_map`` [B * S]: packed row of every token, -1 if masked.
+
+    A row without any unmasked token packs as S tokens (the padded attention computes it with every key valid).
+    ``D * S`` must cover the pad tail ``T_cap - T`` (:func:`bert_pytorch_b200.models.fused.token_bucket`)."""
+    B, S = input_mask.shape
+    dev = input_mask.device
+
+    def i32(t):
+        return t.reshape(B, S).to(torch.int32).contiguous()
+    ids = torch.empty(T_cap, dtype=torch.int32, device=dev)
+    seg, pos = torch.empty_like(ids), torch.empty_like(ids)
+    cu = torch.empty(B + D + 1, dtype=torch.int32, device=dev)
+    cls = torch.empty(B, dtype=torch.int32, device=dev)
+    row_map = torch.empty(B * S, dtype=torch.int32, device=dev)
+    extension().pack_tokens(i32(input_mask), i32(input_ids), None if segment_ids is None else i32(segment_ids),
+                            T_cap, D, ids, seg, pos, cu, cls, row_map)
+    _count()
+    return ids, seg, pos, cu, cls, row_map
 
 
 def gather_rows(src: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:

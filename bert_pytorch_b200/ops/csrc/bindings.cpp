@@ -291,11 +291,56 @@ void embedding_bwd_scatter(Tensor de, Tensor ids, c10::optional<Tensor> seg, Ten
                               opt_pos_ids(pos_ids, ids));
 }
 
-void mlm_compact(Tensor labels, int64_t max_pred, Tensor idx, Tensor tgt, Tensor count) {
+inline void check_i32(const Tensor& t, const Tensor& like, int64_t numel, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.device() == like.device(), name, " must be a CUDA tensor on the device of the batch");
+  TORCH_CHECK(t.scalar_type() == at::kInt && t.is_contiguous() && t.numel() == numel, name, " must be a contiguous int32 "
+              "tensor of ", numel, " elements");
+}
+
+// row_map (optional, int32 [B*S], from pack_tokens): idx gets packed rows, labels of masked tokens are dropped
+void mlm_compact(Tensor labels, int64_t max_pred, Tensor idx, Tensor tgt, Tensor count, c10::optional<Tensor> row_map) {
   TORCH_CHECK(labels.scalar_type() == at::kInt && labels.dim() == 2 && labels.is_contiguous(), "labels: int32 [B,S]");
+  const int* rm = nullptr;
+  if (row_map.has_value() && row_map->defined()) {
+    TORCH_CHECK(labels.is_cuda(), "labels must be a CUDA tensor");
+    check_i32(*row_map, labels, labels.numel(), "row_map");
+    check_i32(idx, labels, labels.size(0) * max_pred, "idx");
+    check_i32(tgt, labels, labels.size(0) * max_pred, "tgt");
+    check_i32(count, labels, 1, "count");
+    rm = row_map->data_ptr<int>();
+  }
   c10::cuda::CUDAGuard guard(labels.device());
   b200::mlm_compact(labels.data_ptr<int>(), (int)labels.size(0), (int)labels.size(1), (int)max_pred,
-                    idx.data_ptr<int>(), tgt.data_ptr<int>(), count.data_ptr<int>(), cur_stream());
+                    idx.data_ptr<int>(), tgt.data_ptr<int>(), count.data_ptr<int>(), cur_stream(), rm);
+}
+
+// Device packing of a [B, S] batch (see pack_tokens_kernel in norm_embed.cu).  mask / ids / seg: int32 [B, S] (seg
+// optional); outputs ids, seg, pos [T_cap], cu [B + D + 1], cls [B], row_map [B * S], all int32.
+void pack_tokens(Tensor mask, Tensor ids_in, c10::optional<Tensor> seg_in, int64_t T_cap, int64_t D, Tensor ids,
+                 Tensor seg, Tensor pos, Tensor cu, Tensor cls, Tensor row_map) {
+  TORCH_CHECK(mask.is_cuda(), "pack_tokens: mask must be a CUDA tensor");
+  TORCH_CHECK(mask.dim() == 2, "pack_tokens: mask must be [B, S]");
+  const int64_t B = mask.size(0), S = mask.size(1);
+  TORCH_CHECK(B >= 1 && B <= b200::pack_tokens_max_batch() && S >= 1, "pack_tokens: 1 <= B <= ",
+              b200::pack_tokens_max_batch(), " and S >= 1");
+  TORCH_CHECK(T_cap >= 1 && D >= 0 && T_cap <= B * S + D * S, "pack_tokens: T_cap in [1, (B + D) * S], D >= 0");
+  check_i32(mask, mask, B * S, "mask");
+  check_i32(ids_in, mask, B * S, "input_ids");
+  const int* seg_p = nullptr;
+  if (seg_in.has_value() && seg_in->defined()) {
+    check_i32(*seg_in, mask, B * S, "segment_ids");
+    seg_p = seg_in->data_ptr<int>();
+  }
+  check_i32(ids, mask, T_cap, "ids");
+  check_i32(seg, mask, T_cap, "seg");
+  check_i32(pos, mask, T_cap, "pos_ids");
+  check_i32(cu, mask, B + D + 1, "cu_seqlens");
+  check_i32(cls, mask, B, "cls_rows");
+  check_i32(row_map, mask, B * S, "row_map");
+  c10::cuda::CUDAGuard guard(mask.device());
+  b200::pack_tokens(mask.data_ptr<int>(), ids_in.data_ptr<int>(), seg_p, (int)B, (int)S, (int)T_cap, (int)D,
+                    ids.data_ptr<int>(), seg.data_ptr<int>(), pos.data_ptr<int>(), cu.data_ptr<int>(),
+                    cls.data_ptr<int>(), row_map.data_ptr<int>(), cur_stream());
 }
 void gather_rows(Tensor src, Tensor idx, Tensor dst) {
   check_bf16(src, "src"); check_bf16(dst, "dst");
@@ -577,7 +622,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("dgelu_bwd", &dgelu_bwd);
   m.def("embedding_fwd", &embedding_fwd);
   m.def("embedding_bwd_scatter", &embedding_bwd_scatter);
-  m.def("mlm_compact", &mlm_compact);
+  m.def("mlm_compact", &mlm_compact, pybind11::arg("labels"), pybind11::arg("max_pred"), pybind11::arg("idx"),
+        pybind11::arg("tgt"), pybind11::arg("count"), pybind11::arg("row_map") = pybind11::none());
+  m.def("pack_tokens", &pack_tokens);
   m.def("gather_rows", &gather_rows);
   m.def("scatter_rows", &scatter_rows);
   m.def("softmax_ce", &softmax_ce);

@@ -27,7 +27,13 @@ void embedding_fwd(const int* ids, const int* seg, const void* word, const void*
 // pos_ids (int32 [M], optional): position row of every token row; without it the position is row % S
 void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float* gword, float* gpos, float* gtype,
                            int M, int S, int H, int type_rows, cudaStream_t st, const int* pos_ids = nullptr);
-void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st);
+// row_map (int32 [B*S], optional): idx gets packed rows, and labels of masked tokens (row_map -1) are dropped
+void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st,
+                 const int* row_map = nullptr);
+// device packing of a [B, S] batch into T_cap rows + D dummy sequences (see pack_tokens_kernel); B <= pack_tokens_max_batch()
+int pack_tokens_max_batch();
+void pack_tokens(const int* mask, const int* ids_in, const int* seg_in, int B, int S, int T_cap, int D, int* ids,
+                 int* seg, int* pos, int* cu, int* cls, int* row_map, cudaStream_t st);
 void gather_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st);
 void scatter_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st);
 

@@ -668,9 +668,12 @@ embed_bwd_postype_kernel(const __nv_bfloat16* __restrict__ de, const int* __rest
 // MLM position compaction: per sequence, the positions with label >= 0 (at most max_pred) are written to
 // idx[b*max_pred + j] (global row index b*S+s), the tail is -1; tgt gets the labels (-1 tail);
 // count accumulates the number of valid targets.  Deterministic order (ascending position).
+// REMAP (unpadded pre-training): idx holds the packed row row_map[b*S+s] instead, and a label whose token is masked
+// (row_map -1) is dropped -- neither written nor counted.
 // ------------------------------------------------------------------------------------------------
+template <bool REMAP>
 __global__ void mlm_compact_kernel(const int* __restrict__ labels, int S, int max_pred, int* __restrict__ idx,
-                                   int* __restrict__ tgt, int* __restrict__ count) {
+                                   int* __restrict__ tgt, int* __restrict__ count, const int* __restrict__ row_map) {
   const int b = blockIdx.x;
   __shared__ int n;
   if (threadIdx.x == 0) n = 0;
@@ -680,12 +683,14 @@ __global__ void mlm_compact_kernel(const int* __restrict__ labels, int S, int ma
   int base = 0;
   for (int s0 = 0; s0 < S; s0 += 32) {
     const int s = s0 + lane;
-    const int lab = s < S ? labels[b * S + s] : -1;
+    int lab = s < S ? labels[b * S + s] : -1;
+    const int row = REMAP && lab >= 0 ? row_map[b * S + s] : b * S + s;
+    if (REMAP && row < 0) lab = -1;
     const unsigned m = __ballot_sync(0xffffffffu, lab >= 0);
     if (lab >= 0) {
       const int j = base + __popc(m & ((1u << lane) - 1));
       if (j < max_pred) {
-        idx[b * max_pred + j] = b * S + s;
+        idx[b * max_pred + j] = row;
         tgt[b * max_pred + j] = lab;
       }
     }
@@ -697,6 +702,94 @@ __global__ void mlm_compact_kernel(const int* __restrict__ labels, int S, int ma
     tgt[b * max_pred + j] = -1;
   }
   if (lane == 0) atomicAdd(count, valid);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Token packing of a [B, S] pre-training batch on the device (no host sync: it runs inside a captured graph).  One CTA;
+// every output has a fixed shape and is written completely on each call:
+//   ids / seg / pos [T_cap]  the T unmasked tokens in b*S+s order (id, segment, position s), then the pad tail rows
+//                            T .. T_cap-1: id 0, segment 0, position = offset inside its dummy sequence
+//   cu [B + D + 1]           the B real sequences, then D dummy sequences of at most S rows that cover the pad tail
+//                            (length 0 where the tail does not need them)
+//   cls [B]                  first packed row of every sequence
+//   row_map [B*S]            packed row of token (b, s), -1 where the token is masked
+// A row without any unmasked token packs as S valid tokens: the padded program computes such a row with every key
+// valid (the attention length-0 rule), so both modes see the same values and cls always points at a real row.  The
+// tail rows are real [PAD] tokens and each tail chunk attends only to itself, so they stay finite and inert.  Nothing
+// is written at or past T_cap: a T_cap below T truncates (the host sizes T_cap and D from the same mask).
+// ------------------------------------------------------------------------------------------------
+constexpr int PACK_THREADS = 512;
+constexpr int PACK_MAX_B = 1024;
+
+__global__ void __launch_bounds__(PACK_THREADS) pack_tokens_kernel(
+    const int* __restrict__ mask, const int* __restrict__ ids_in, const int* __restrict__ seg_in, int B, int S,
+    int T_cap, int D, int* __restrict__ ids, int* __restrict__ seg, int* __restrict__ pos, int* __restrict__ cu,
+    int* __restrict__ cls, int* __restrict__ row_map) {
+  __shared__ int off[PACK_MAX_B + 1];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+  // 1. packed length of every sequence (warp per row)
+  for (int b = warp; b < B; b += warps) {
+    int n = 0;
+    for (int s0 = 0; s0 < S; s0 += 32) {
+      const int s = s0 + lane;
+      n += __popc(__ballot_sync(0xffffffffu, s < S && mask[(size_t)b * S + s] != 0));
+    }
+    if (lane == 0) off[b + 1] = n > 0 ? n : S;
+  }
+  __syncthreads();
+  // 2. inclusive scan of the lengths (warp 0) -> off[b] = first packed row of sequence b, off[B] = T
+  if (warp == 0) {
+    int carry = 0;
+    for (int b0 = 0; b0 < B; b0 += 32) {
+      const int b = b0 + lane;
+      int v = b < B ? off[b + 1] : 0;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, v, d);
+        if (lane >= d) v += t;
+      }
+      if (b < B) off[b + 1] = v + carry;
+      carry += __shfl_sync(0xffffffffu, v, 31);
+    }
+    if (lane == 0) off[0] = 0;
+  }
+  __syncthreads();
+  const int T = min(off[B], T_cap);
+  // 3. the real tokens (warp per row, ordered compaction with ballots); a full-length row keeps every token, which
+  //    covers the empty rows
+  for (int b = warp; b < B; b += warps) {
+    const bool all = off[b + 1] - off[b] == S;
+    int base = off[b];
+    for (int s0 = 0; s0 < S; s0 += 32) {
+      const int s = s0 + lane;
+      const size_t i = (size_t)b * S + s;
+      const bool keep = s < S && (all || mask[i] != 0);
+      const unsigned m = __ballot_sync(0xffffffffu, keep);
+      if (s < S) {
+        const int r = keep ? base + __popc(m & ((1u << lane) - 1)) : -1;
+        const bool in = r >= 0 && r < T_cap;
+        row_map[i] = in ? r : -1;
+        if (in) {
+          ids[r] = ids_in[i];
+          seg[r] = seg_in != nullptr ? seg_in[i] : 0;
+          pos[r] = s;
+        }
+      }
+      base += __popc(m);
+    }
+    if (lane == 0) {
+      cu[b] = min(off[b], T_cap);
+      cls[b] = min(off[b], T_cap - 1);
+    }
+  }
+  // 4. the pad tail and its dummy sequences
+  for (int r = T + threadIdx.x; r < T_cap; r += blockDim.x) {
+    ids[r] = 0;
+    seg[r] = 0;
+    pos[r] = (r - T) % S;
+  }
+  if (threadIdx.x == 0) cu[B] = T;
+  for (int j = threadIdx.x; j < D; j += blockDim.x) cu[B + 1 + j] = (int)min((long long)T_cap, T + (long long)(j + 1) * S);
 }
 
 // rows[i] = src[idx[i]] (zeros when idx < 0)
@@ -885,9 +978,20 @@ void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float
                                                    pos_ids);
 }
 
-void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st) {
+void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st,
+                 const int* row_map) {
   B200_CUDA_CHECK(cudaMemsetAsync(count, 0, sizeof(int), st));
-  mlm_compact_kernel<<<B, 32, 0, st>>>(labels, S, max_pred, idx, tgt, count);
+  if (row_map != nullptr)
+    mlm_compact_kernel<true><<<B, 32, 0, st>>>(labels, S, max_pred, idx, tgt, count, row_map);
+  else
+    mlm_compact_kernel<false><<<B, 32, 0, st>>>(labels, S, max_pred, idx, tgt, count, nullptr);
+}
+
+int pack_tokens_max_batch() { return PACK_MAX_B; }
+
+void pack_tokens(const int* mask, const int* ids_in, const int* seg_in, int B, int S, int T_cap, int D, int* ids,
+                 int* seg, int* pos, int* cu, int* cls, int* row_map, cudaStream_t st) {
+  pack_tokens_kernel<<<1, PACK_THREADS, 0, st>>>(mask, ids_in, seg_in, B, S, T_cap, D, ids, seg, pos, cu, cls, row_map);
 }
 
 void gather_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st) {

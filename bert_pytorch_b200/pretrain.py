@@ -12,7 +12,7 @@ Function names, flags, output files and checkpoint layout follow the reference
   * the loss stays on the device between micro-steps (the reference syncs the host every
     micro-step, run_pretraining.py:542); data arrives through the batched pinned loader;
   * new flags: ``--bf16`` (default compute type on CUDA), ``--fp8``, ``--backend``,
-    ``--device``, ``--no_fused``, ``--loader_depth``.
+    ``--device``, ``--no_fused``, ``--loader_depth``, ``--unpad``.
 Documented deviations from reference quirks: Q7 (first update used acc+1 micro-batches) and
 Q9/Q10 (throughput accounting) are fixed; Q6 (sampler index ran ahead of consumption) is
 fixed by the loader; the rest of the arithmetic (ceil-based accumulation, step numbering of
@@ -38,6 +38,7 @@ from .data import BatchedPretrainingLoader, DistributedSampler, ShardedPretraini
 from .data.tokenization import get_bpe_tokenizer, get_wordpiece_tokenizer
 from .models import BertPretrainingCriterion  # noqa: F401  (public name of run_pretraining.py:96)
 from .models.arena import NO_DECAY_KEYS, ParamArena
+from .models.fused import packed_tokens
 from .optim import GradScaler, Lamb, LinearWarmUpScheduler, PolyWarmUpScheduler
 from .parallel import DataParallel, make_comm, unwrap
 from .utils import checkpoint as ckpt_utils
@@ -99,6 +100,9 @@ def build_parser() -> argparse.ArgumentParser:
                    help="fp8 GEMM operands in the fused engine (e4m3 activations/weights, e5m2 gradients, "
                         "per-tensor delayed scaling); LayerNorm, attention, master weights unchanged")
     p.add_argument("--loader_depth", type=int, default=4)
+    p.add_argument("--unpad", default=False, action="store_true",
+                   help="fused engine: compute only the unmasked tokens of each micro-batch (packed on the device into "
+                        "one of 16 token buckets, one CUDA graph per bucket); fp8 operands run padded")
     return p
 
 
@@ -184,6 +188,7 @@ def prepare_model(args):
 
     model.to(args.device_obj)
     model.checkpoint_activations(args.checkpoint_activations)
+    model.bert.unpad = bool(getattr(args, "unpad", False))      # fused engine only; the PyTorch path ignores it
     if args.no_fused:
         model.enable_apex(False)
     config.max_predictions_per_seq = args.max_predictions_per_seq    # static MLM row capacity of the fused head
@@ -329,8 +334,10 @@ def take_optimizer_step(optimizer, preconditioner, model, scaler):
     optimizer.zero_grad()        # arena: one memset; keeps the persistent grad views alive
 
 
-def forward_backward_pass(model, criterion, scaler, batch, divisor, sync_grads=True, compute_dtype=None):
-    """One micro-step.  Returns the (unscaled, already divided) loss as a device tensor."""
+def forward_backward_pass(model, criterion, scaler, batch, divisor, sync_grads=True, compute_dtype=None, tokens=None):
+    """One micro-step.  Returns the (unscaled, already divided) loss as a device tensor.  ``tokens``: packed token
+    count of the batch (:func:`~.models.fused.packed_tokens` of its mask) for the unpadded fused engine; without it
+    that engine counts on the device (one host sync)."""
     input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels = batch
     base = unwrap(model)
     engine = base.pretrain_engine() if hasattr(base, "pretrain_engine") else None
@@ -346,7 +353,7 @@ def forward_backward_pass(model, criterion, scaler, batch, divisor, sync_grads=T
         engine.grad_push = bool(push)       # last micro-step: weight-gradient GEMMs reduce-scatter over NVLink
         try:
             loss = engine.forward_backward(input_ids, segment_ids, input_mask, masked_lm_labels,
-                                           next_sentence_labels, grad_scale=loss_scale / divisor)
+                                           next_sentence_labels, grad_scale=loss_scale / divisor, tokens=tokens)
         finally:
             if push:
                 comm.end_push()
@@ -431,12 +438,14 @@ def main(args) -> Tuple[int, float]:
     while not done:
         sampler.set_epoch(epoch)
         for batch in loader:
+            # --unpad: the token count comes from the pinned host mask (no device read-back)
+            tokens = packed_tokens(batch[2]) if args.unpad else None
             batch = [t.to(device, non_blocking=True) for t in batch]
             micro += 1
             sync = micro == acc
             with nvtx_range("micro_step_sync" if sync else "micro_step"):
                 loss = forward_backward_pass(model, criterion, scaler, batch, acc, sync_grads=sync,
-                                             compute_dtype=args.compute_dtype)
+                                             compute_dtype=args.compute_dtype, tokens=tokens)
             window_loss += loss
             last_loss = loss
             session_seqs += batch[0].size(0)
