@@ -19,6 +19,7 @@ import torch
 from torch.utils.data import DataLoader
 
 from . import models as modeling
+from . import ops
 from .config import BertConfig
 from .data.ner import NERDataset
 from .data.tokenization import get_bpe_tokenizer, get_wordpiece_tokenizer
@@ -48,6 +49,10 @@ def parse_arguments(argv=None):
     p.add_argument("--unpad", action="store_true", default=False,
                    help="with --bf16: the fused engine computes only the unmasked tokens, in training and evaluation "
                         "(exact: the loss and F1 read unmasked positions only) (new)")
+    p.add_argument("--deterministic", action="store_true", default=False,
+                   help="bitwise-reproducible training: the fused engine's fixed-order reductions (no floating-point "
+                        "atomics) and torch.use_deterministic_algorithms(True); the same program on the same inputs, GPU "
+                        "and build gives the same loss, gradients and weights (new)")
     args = p.parse_args(argv)
     args.cuda = torch.cuda.is_available() and not args.no_cuda
     return args
@@ -149,6 +154,8 @@ def evaluate(model, loader, args) -> Tuple[float, float]:
 
 def main(argv=None) -> Dict[str, float]:
     args = parse_arguments(argv)
+    if args.deterministic:
+        ops.use_deterministic()
     random.seed(args.seed); np.random.seed(args.seed); torch.manual_seed(args.seed)
     config = BertConfig.from_json_file(args.model_config_file)
     config.pad_vocab(8)

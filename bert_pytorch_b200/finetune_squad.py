@@ -35,6 +35,7 @@ from torch.utils.data import DataLoader, RandomSampler, SequentialSampler, Tenso
 from torch.utils.data.distributed import DistributedSampler as TorchDistributedSampler
 
 from . import models as modeling
+from . import ops
 from .config import BertConfig
 from .data import squad as SQ
 from .data.squad import (  # noqa: F401  (public helpers of run_squad.py, implemented in data/squad.py)
@@ -100,6 +101,10 @@ def build_parser() -> argparse.ArgumentParser:
                    help="prediction through the fused engine computes only the unmasked tokens. Training stays padded: "
                         "the start / end cross-entropy normalises over every position, padded ones included, so an "
                         "unpadded training step would not be exact")
+    p.add_argument("--deterministic", default=False, action="store_true",
+                   help="bitwise-reproducible training: the fused engine's fixed-order reductions (no floating-point "
+                        "atomics) and torch.use_deterministic_algorithms(True); the same program on the same inputs, GPU "
+                        "and build gives the same loss, gradients and weights")
     return p
 
 
@@ -126,6 +131,8 @@ def squad_loss(start_logits, end_logits, start_positions, end_positions):
 
 def main(argv=None) -> dict:
     args = build_parser().parse_args(argv)
+    if args.deterministic:
+        ops.use_deterministic()
     args.fp16 = args.fp16 or args.amp
     with open(args.config_file) as f:
         model_json = json.load(f)

@@ -789,7 +789,7 @@ class FusedPretrainer:
         key = (tuple(input_ids.shape), self.model.training, next_sentence_labels is not None,
                segment_ids is not None, tuple(str(t.dtype) for t in args if t is not None),
                bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)), self.engine.fp8,
-               bool(self.grad_push), bool(self.engine.wgrad_side), bucket)
+               bool(self.grad_push), bool(self.engine.wgrad_side), K.deterministic(), bucket)
         ent = self._graphs.setdefault(key, {"calls": 0})
         ent["calls"] += 1
         eng = self.engine
@@ -911,7 +911,11 @@ class FusedPretrainer:
             K.wgrad_accumulate(d_z, cls_tok, pool.weight.grad)
             K.colsum_accumulate(d_z, pool.bias.grad)
             d_cls = K.gemm(d_z, pw, layout=K.NN)
-            if pk is not None:                     # the same bf16 add at the (distinct) first packed rows
+            if pk is not None and K.deterministic():
+                # torch's deterministic index_add_ sorts its indices; the rows are distinct, so gather, add and scatter
+                # back instead: the same bf16 add, on the engine's kernels
+                K.scatter_rows(K.gather_rows(d_seq, pk.cls_rows) + d_cls, pk.cls_rows, d_seq)
+            elif pk is not None:                   # the same bf16 add at the (distinct) first packed rows
                 d_seq.index_add_(0, pk.cls_rows.long(), d_cls)
             else:
                 d_seq.view(B, S, H)[:, 0] += d_cls

@@ -23,6 +23,24 @@ NUM_SMS = 132           # H100 SXM; only the tile heuristics below use it (the k
 KERNEL_LAUNCHES = 0     # every wrapper bumps this: bench.py reports it as ``gpu_launches``
 
 
+def deterministic() -> bool:
+    """Deterministic mode: the wrappers below take fixed-order forms of every floating-point sum whose order would
+    otherwise depend on CTA scheduling (split-K weight gradients, bias gradients, attention dQ, the embedding scatter,
+    the losses, the optimizer norms), so that the same program on the same inputs, GPU and build gives the same bits.
+    On with ``B200_DETERMINISTIC=1`` or ``torch.use_deterministic_algorithms(True)``."""
+    return os.environ.get("B200_DETERMINISTIC", "0") == "1" or torch.are_deterministic_algorithms_enabled()
+
+
+def use_deterministic() -> None:
+    """What the runners' ``--deterministic`` does, before CUDA starts: torch's flag (which also switches this module
+    into deterministic mode) and the cuBLAS workspace setting it needs for the torch ops around the engine (fine-tuning
+    heads, cross-entropy).  torch's fill of uninitialised memory stays off: every engine output and workspace is written
+    in full before it is read, so the fill would only cost a memset per allocation."""
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+    torch.use_deterministic_algorithms(True)
+    torch.utils.deterministic.fill_uninitialized_memory = False
+
+
 def pick_block_n(M: int, N: int, epi: int = EPI_NONE) -> int:
     """The tile width :func:`gemm` chooses for an [M, N] output with epilogue ``epi`` (128 x 256 or 128 x 128
     tiles)."""
@@ -68,7 +86,14 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, layout: int = NT, epi: int = EPI_N
     ``colsum`` (fp32 [N], EPI_NONE / EPI_ADD / EPI_MUL): accumulates the column sums of the bf16 output (a bias
     gradient that would otherwise need its own pass over the tensor).  ``mask_out`` (uint8 [M, N / 8],
     EPI_BIAS_DROP_RES): receives the dropout keep bits, which :func:`layer_norm_bwd` can read
-    back (``keep_mask``) instead of regenerating them."""
+    back (``keep_mask``) instead of regenerating them.
+    Deterministic mode: EPI_ACCUM_F32 runs without split-K (:func:`wgrad_accumulate` splits in order itself), and
+    ``colsum`` is a separate fixed-order column sum of the output (the same bf16 values the epilogue would have
+    summed)."""
+    det = deterministic()
+    if det:
+        k_splits = 1 if epi == EPI_ACCUM_F32 else k_splits
+        colsum, det_colsum = None, colsum
     if layout == NT:
         M, N = a.size(0), b.size(0)
     elif layout == NN:
@@ -83,6 +108,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, layout: int = NT, epi: int = EPI_N
     extension().gemm(a, b, out, layout, epi, bias, res, aux_out, k_splits, block_n, alpha, p_drop, seed, stream,
                      scale_a, scale_b, a_e5m2, b_e5m2, push, colsum, mask_out, mask_in)
     _count()
+    if det and det_colsum is not None:
+        colsum_accumulate(out, det_colsum)
     return out
 
 
@@ -146,6 +173,24 @@ def wgrad_accumulate(dy: torch.Tensor, x: torch.Tensor, grad: torch.Tensor, alph
     n_out, k_out = grad.shape
     bn = 256 if k_out >= 256 else _pick_block_n(n_out, k_out)
     splits = wgrad_splits(n_out, k_out, dy.size(0) // (2 if fp8 else 1), bn)
+    if splits > 1 and deterministic():
+        if extension().grad_peers_world() > 1:
+            # the gradient arenas are registered with the peer-memory backend: peers add into this arena and the GEMMs
+            # push tiles to their owners, which a plain read-modify-write of the partials would race with
+            raise RuntimeError("deterministic mode covers one GPU; it cannot run with the peer-memory gradient backend "
+                               "(--backend fused)")
+        # the split-K partition done in order: each range of 128-row blocks of the reduction is stored plainly to its
+        # own fp32 partial, and the partials are added to the gradient in range order.  (Not one split: an fp8 wgmma
+        # accumulates with less than fp32 precision, so the whole reduction in one pass would lose accuracy.)
+        M = dy.size(0)
+        step = -(-M // (splits * 128)) * 128
+        parts = torch.empty(-(-M // step), n_out, k_out, dtype=torch.float32, device=grad.device)
+        for s in range(parts.size(0)):
+            gemm(dy[s * step:(s + 1) * step], x[s * step:(s + 1) * step], layout=TN, epi=EPI_F32, out=parts[s],
+                 block_n=bn, alpha=alpha, **fp8)
+        extension().ordered_sum(parts, grad)
+        _count()
+        return
     # ``push``: with the peer-memory backend in push mode the tiles go to the owner rank's arena (GEMM -> reduce-scatter)
     gemm(dy, x, layout=TN, epi=EPI_ACCUM_F32, out=grad, block_n=bn, alpha=alpha, k_splits=splits, push=push, **fp8)
 
@@ -213,15 +258,16 @@ def layer_norm_bwd(dy: torch.Tensor, x: torch.Tensor, mean: torch.Tensor, rstd: 
     M, H = x.numel() // x.size(-1), x.size(-1)
     q, rec, e5 = _fp8_side(fp8 if want_dropped else None, x)
     extension().layer_norm_bwd(dy, x, mean, rstd, gamma, dx, dxd, dgamma, dbeta, dbias, _ln_workspace(M, H, x.device),
-                               p_drop, seed, drop_stream, in_stream, q, rec, e5, keep_mask)
+                               p_drop, seed, drop_stream, in_stream, q, rec, e5, keep_mask, deterministic())
     _count(2)
     return (dx, dxd) if fp8 is None else (dx, dxd, q)
 
 
 def colsum_accumulate(x: torch.Tensor, out: torch.Tensor) -> None:
     """out[N] (fp32) += x[M,N].sum(0)"""
-    extension().colsum(x, out)
-    _count()
+    det = deterministic()
+    extension().colsum(x, out, det)
+    _count(2 if det else 1)
 
 
 def gelu_fwd(x: torch.Tensor, fp8=None):
@@ -233,11 +279,13 @@ def gelu_fwd(x: torch.Tensor, fp8=None):
 
 
 def dgelu_bwd(dy: torch.Tensor, x: torch.Tensor, dbias: Optional[torch.Tensor] = None, fp8=None):
-    """dy * gelu'(x); ``dbias`` (fp32 [N]) accumulates the column sums of the result."""
+    """dy * gelu'(x); ``dbias`` (fp32 [N]) accumulates the column sums of the result (of its fp32 values, before the
+    bf16 rounding; deterministic mode: per-block sums finished in a fixed order)."""
     dx = torch.empty_like(dy)
     q, rec, e5 = _fp8_side(fp8, dy)
-    extension().dgelu_bwd(dy, x, dx, dbias, q, rec, e5)
-    _count()
+    det = deterministic() and dbias is not None
+    extension().dgelu_bwd(dy, x, dx, dbias, q, rec, e5, det)
+    _count(2 if det else 1)
     return dx if fp8 is None else (dx, q)
 
 
@@ -257,8 +305,11 @@ def embedding_fwd(ids, seg, word, pos, type_emb, gamma, beta, S: int, *, eps=1e-
 
 
 def embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S: int, *, pos_ids: Optional[torch.Tensor] = None) -> None:
-    extension().embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S, pos_ids)
-    _count()
+    """Deterministic mode: the rows are sorted by table row and every table row is summed by one owner in token order
+    (32768 token rows at a time, the chunks added in order)."""
+    det = deterministic()
+    extension().embedding_bwd_scatter(de, ids, seg, gword, gpos, gtype, S, pos_ids, det)
+    _count(9 if det else 2)
 
 
 def mlm_compact(labels: torch.Tensor, max_pred: int, row_map: Optional[torch.Tensor] = None):
@@ -322,16 +373,18 @@ def nsp_head_(pooled: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, labels:
     ``dw`` / ``db`` (fp32) accumulate the classifier gradients, returns dz = d loss / d (pooler pre-activation) [B,H]
     bf16 (tanh' of the pooler folded in)."""
     dz = torch.empty_like(pooled)
-    extension().nsp_head(pooled, w, bias, labels, grad_scale, loss_out, dz, dw, db)
-    _count()
+    det = deterministic()
+    extension().nsp_head(pooled, w, bias, labels, grad_scale, loss_out, dz, dw, db, det)
+    _count(4 if det else 1)
     return dz
 
 
 def softmax_ce_(logits: torch.Tensor, targets: torch.Tensor, count: torch.Tensor, grad_scale: float,
                 loss_out: torch.Tensor) -> None:
     """In place: logits <- d loss / d logits (scaled); loss_out += mean CE over valid targets."""
-    extension().softmax_ce(logits, targets, count, grad_scale, loss_out)
-    _count()
+    det = deterministic()
+    extension().softmax_ce(logits, targets, count, grad_scale, loss_out, det)
+    _count(2 if det else 1)
 
 
 def _attn_shape(qkv: torch.Tensor, seqlens, cu_seqlens, S):
@@ -371,10 +424,13 @@ def attention_bwd(qkv, seqlens, ctx, dctx, lse, heads: int, *, p_drop=0.0, seed=
     B, S, rows, H = _attn_shape(qkv, seqlens, cu_seqlens, S)
     dqkv = torch.empty_like(qkv)
     delta = torch.empty(B, heads, S, dtype=torch.float32, device=qkv.device)
-    dq_acc = torch.empty(rows, H, dtype=torch.float32, device=qkv.device)
+    # deterministic mode with more than one 128-key block: one dQ slice per key block, summed in key-block order
+    det = deterministic()
+    slices = (S + 127) // 128 if det and S > 128 else 1
+    dq_acc = torch.empty(slices, rows, H, dtype=torch.float32, device=qkv.device)
     q, rec, e5 = _fp8_side(fp8, dqkv)
     extension().attention_bwd(qkv, seqlens, ctx, dctx, lse, dqkv, delta, dq_acc, heads, 1.0 / math.sqrt(H // heads), p_drop,
-                              seed, stream, q, rec, e5, cu_seqlens, S)
+                              seed, stream, q, rec, e5, cu_seqlens, S, det)
     _count(2)
     return dqkv if fp8 is None else (dqkv, q)
 
@@ -415,6 +471,7 @@ def multi_tensor_l2norm(tensors: List[torch.Tensor], per_tensor: bool = False):
     dev = tensors[0].device
     total = torch.zeros(1, dtype=torch.float32, device=dev)
     per = torch.zeros(len(tensors), dtype=torch.float32, device=dev) if per_tensor else None
+    det = deterministic()
     by_dtype: Dict[torch.dtype, List[int]] = {}
     for i, t in enumerate(tensors):
         if not t.is_contiguous():
@@ -424,8 +481,8 @@ def multi_tensor_l2norm(tensors: List[torch.Tensor], per_tensor: bool = False):
         group = [tensors[i] for i in idxs]
         ptrs, ct, cs, cl = _list_tables(group)
         sub = torch.zeros(len(group), dtype=torch.float32, device=dev) if per_tensor else None
-        extension().mt_l2norm(_DT[dt], ptrs, ct, cs, cl, sub, total)
-        _count()
+        extension().mt_l2norm(_DT[dt], ptrs, ct, cs, cl, sub, total, det)
+        _count(1 + (per_tensor + 1 if det else 0))
         if per_tensor:
             per[torch.tensor(idxs, device=dev)] = sub
     return total.sqrt().squeeze(0), (per.sqrt() if per_tensor else torch.zeros(0, device=dev))
@@ -500,13 +557,14 @@ def arena_lamb_step(arena, optimizer, inv_scale=None, found_inf=None) -> None:
     ext = extension()
     inv = inv_scale.reshape(1) if inv_scale is not None else None
     fi = found_inf.reshape(1) if found_inf is not None else None
-    ext.flat_sumsq(arena.flat_grad, inv, T["stats"], fi)
+    det = deterministic()
+    ext.flat_sumsq(arena.flat_grad, inv, T["stats"], fi, det)
     ext.arena_lamb(arena.flat_grad, arena.flat_param, arena.exp_avg, arena.exp_avg_sq, arena.flat_shadow, T["ct"],
                    T["cs"], T["cl"], T["decay"], T["stats"], T["norms"], inv, fi, float(lr), float(b1), float(b2),
                    float(eps), float(wd), step, bool(_uniform(optimizer, "bias_correction")),
                    bool(_uniform(optimizer, "grad_averaging")), float(_uniform(optimizer, "max_grad_norm") or 0.0),
-                   bool(optimizer.adam_w_mode), bool(optimizer.use_nvlamb))
-    _count(3)
+                   bool(optimizer.adam_w_mode), bool(optimizer.use_nvlamb), det)
+    _count(5 if det else 3)
     # apex semantics: the step counter only advances when the update was applied.  Keeping that exact
     # would need a host sync on found_inf; with a scaler we advance optimistically only when no scaler
     # is in play, otherwise we read the flag (fp16 path only -- bf16 never has a scaler).

@@ -318,10 +318,13 @@ __device__ __forceinline__ uint32_t tile_pair_offset(int r, int g, int c) {
 constexpr int ATT_BWD_THREADS = 256;
 constexpr int ATT_BWD_SMEM = 16384 * 2 + 8192 * 8 + 1024 + 64;
 
-template <bool VARLEN>
-__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
-                const __grid_constant__ CUtensorMap tmap_do, const AttnArgs p) {
+// SLICED (deterministic mode): key block kb adds its dQ into its own fp32 slice dq_acc + kb * slice, which
+// attn_dq_convert_kernel<true> sums in key-block order.  The two warpgroups of a CTA add onto a zeroed slice, and
+// 0 + a + b == 0 + b + a exactly, so each slice is order-free.  For the same reason a single key block (S <= 128)
+// needs no slices: attn_bwd_kernel is deterministic there as it is.
+template <bool VARLEN, bool SLICED>
+__device__ __forceinline__ void attn_bwd_body(const CUtensorMap& tmap_q, const CUtensorMap& tmap_kv,
+                                              const CUtensorMap& tmap_do, const AttnArgs& p, size_t slice) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = smem;                        // 16 KB: 128 keys, warpgroup w reads rows [64 w, 64 w + 64)
@@ -454,6 +457,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       const int q = i * QT + r_lo + 8 * h;
       if (q < q_end) {
         float* dst = p.dq_acc + (size_t)(row0 + q) * p.H + head * HD + 2 * c;
+        if constexpr (SLICED) dst += kb * slice;
 #pragma unroll
         for (int g = 0; g < 8; ++g)
           asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * g), "f"(dq[4 * g + 2 * h]),
@@ -472,9 +476,25 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   if (p.f8.q) fp8_amax_commit(p.f8, amax);
 }
 
-// dq_acc (fp32 [B*S, H]) -> q slots of dqkv (bf16 [B*S, 3H])
-__global__ void __launch_bounds__(256)
-attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dqkv, long long rows, int H, const Fp8Out f8) {
+template <bool VARLEN>
+__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
+                const __grid_constant__ CUtensorMap tmap_do, const AttnArgs p) {
+  attn_bwd_body<VARLEN, false>(tmap_q, tmap_kv, tmap_do, p, 0);
+}
+
+template <bool VARLEN>
+__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
+attn_bwd_sliced_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
+                       const __grid_constant__ CUtensorMap tmap_do, const AttnArgs p, long long slice) {
+  attn_bwd_body<VARLEN, true>(tmap_q, tmap_kv, tmap_do, p, (size_t)slice);
+}
+
+// dq_acc (fp32 [B*S, H]) -> q slots of dqkv (bf16 [B*S, 3H]).  SLICED: dq_acc is [nslices, rows, H], summed in slice
+// order (a varlen CTA past the end of its sequence leaves its slice zero).
+template <bool SLICED>
+__device__ __forceinline__ void attn_dq_convert_body(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dqkv,
+                                                     long long rows, int H, const Fp8Out& f8, int nslices) {
   const int per_row = H / 8;
   const float qscale = f8.q ? f8.meta[1] : 0.f;
   float amax = 0.f;
@@ -482,8 +502,16 @@ attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict_
        i += (long long)gridDim.x * blockDim.x) {
     const long long row = i / per_row;
     const int col = (int)(i % per_row) * 8;
-    const float4 a = *reinterpret_cast<const float4*>(acc + row * H + col);
-    const float4 c = *reinterpret_cast<const float4*>(acc + row * H + col + 4);
+    float4 a = *reinterpret_cast<const float4*>(acc + row * H + col);
+    float4 c = *reinterpret_cast<const float4*>(acc + row * H + col + 4);
+    if constexpr (SLICED) {
+      for (int k = 1; k < nslices; ++k) {
+        const float* sl = acc + (size_t)k * rows * H + row * H + col;
+        const float4 a2 = *reinterpret_cast<const float4*>(sl), c2 = *reinterpret_cast<const float4*>(sl + 4);
+        a.x += a2.x; a.y += a2.y; a.z += a2.z; a.w += a2.w;
+        c.x += c2.x; c.y += c2.y; c.z += c2.z; c.w += c2.w;
+      }
+    }
     *reinterpret_cast<uint4*>(dqkv + row * 3 * H + col) =
         make_uint4(pack_bf16(a.x, a.y), pack_bf16(a.z, a.w), pack_bf16(c.x, c.y), pack_bf16(c.z, c.w));
     if (f8.q) {
@@ -492,6 +520,17 @@ attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict_
     }
   }
   if (f8.q) fp8_amax_commit(f8, amax);
+}
+
+__global__ void __launch_bounds__(256)
+attn_dq_convert_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dqkv, long long rows, int H, const Fp8Out f8) {
+  attn_dq_convert_body<false>(acc, dqkv, rows, H, f8, 1);
+}
+
+__global__ void __launch_bounds__(256)
+attn_dq_convert_sliced_kernel(const float* __restrict__ acc, __nv_bfloat16* __restrict__ dqkv, long long rows, int H,
+                              const Fp8Out f8, int nslices) {
+  attn_dq_convert_body<true>(acc, dqkv, rows, H, f8, nslices);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -533,39 +572,47 @@ void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, i
 
 template <bool VARLEN>
 static void launch_bwd(const void* qkv, const void* ctx, const void* dctx, const AttnArgs& a, long long rows,
-                       cudaStream_t st) {
+                       cudaStream_t st, bool deterministic) {
   const int B = a.B, S = a.S, h = a.h, H = a.H;
+  const int nkb = (S + KT - 1) / KT;
+  const bool sliced = deterministic && nkb > 1;           // dq_acc then holds nkb slices of [rows, H]
   const long long groups = (long long)B * S * h;
   attn_delta_kernel<VARLEN><<<(unsigned)((groups * 8 + 255) / 256), 256, 0, st>>>(
       (const __nv_bfloat16*)ctx, (const __nv_bfloat16*)dctx, const_cast<float*>(a.delta), B, S, h, H, a.seqlens);
-  B200_CUDA_CHECK(cudaMemsetAsync(a.dq_acc, 0, sizeof(float) * (size_t)rows * H, st));
+  B200_CUDA_CHECK(cudaMemsetAsync(a.dq_acc, 0, sizeof(float) * (size_t)(sliced ? nkb : 1) * rows * H, st));
   CUtensorMap tq = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, QT);
   CUtensorMap tkv = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, KT);
   CUtensorMap td = make_tmap_2d_bf16(dctx, H, (uint64_t)rows, H, 64, QT);
   static bool once = false;
   if (!once) {
     B200_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_BWD_SMEM));
+    B200_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_sliced_kernel<VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ATT_BWD_SMEM));
     once = true;
   }
-  attn_bwd_kernel<VARLEN><<<dim3((S + KT - 1) / KT, B * h), ATT_BWD_THREADS, ATT_BWD_SMEM, st>>>(tq, tkv, td, a);
+  if (sliced)
+    attn_bwd_sliced_kernel<VARLEN><<<dim3(nkb, B * h), ATT_BWD_THREADS, ATT_BWD_SMEM, st>>>(tq, tkv, td, a, rows * H);
+  else
+    attn_bwd_kernel<VARLEN><<<dim3(nkb, B * h), ATT_BWD_THREADS, ATT_BWD_SMEM, st>>>(tq, tkv, td, a);
   const long long work = rows * (H / 8);
   int g = (int)((work + 255) / 256);
   if (g > num_sms() * 16) g = num_sms() * 16;
-  attn_dq_convert_kernel<<<g, 256, 0, st>>>(a.dq_acc, a.dqkv, rows, H, a.f8);
+  if (sliced) attn_dq_convert_sliced_kernel<<<g, 256, 0, st>>>(a.dq_acc, a.dqkv, rows, H, a.f8, nkb);
+  else attn_dq_convert_kernel<<<g, 256, 0, st>>>(a.dq_acc, a.dqkv, rows, H, a.f8);
 }
 
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
                    Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
-                   const int* cu_seqlens, long long T) {
+                   const int* cu_seqlens, long long T, bool deterministic) {
   AttnArgs a;
   fill_args(a, B, S, h, d, cu_seqlens ? cu_seqlens : seqlens, scale, seed, stream, p_drop);
   a.f8 = f8;
   a.lse = const_cast<float*>(lse); a.delta = delta_ws; a.dqkv = (__nv_bfloat16*)dqkv; a.dq_acc = dq_acc;
   a.ctx = (__nv_bfloat16*)const_cast<void*>(ctx);
   if (dq_acc == nullptr) { fprintf(stderr, "[b200] attention_bwd needs a dq accumulation buffer\n"); abort(); }
-  if (cu_seqlens) launch_bwd<true>(qkv, ctx, dctx, a, T, st);
-  else launch_bwd<false>(qkv, ctx, dctx, a, (long long)B * S, st);
+  if (cu_seqlens) launch_bwd<true>(qkv, ctx, dctx, a, T, st, deterministic);
+  else launch_bwd<false>(qkv, ctx, dctx, a, (long long)B * S, st, deterministic);
 }
 
 }  // namespace b200

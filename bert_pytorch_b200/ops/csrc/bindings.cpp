@@ -12,6 +12,11 @@ namespace {
 using torch::Tensor;
 
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
+// fp32 workspace of a deterministic-mode kernel chain, from the caching allocator on the current stream (stream-ordered:
+// it is only reused by work queued after the chain)
+inline Tensor f32_workspace(const Tensor& like, int64_t n) {
+  return at::empty({std::max<int64_t>(n, 1)}, like.options().dtype(at::kFloat));
+}
 inline void check_bf16(const Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
   TORCH_CHECK(t.scalar_type() == at::kBFloat16, name, " must be bf16");
@@ -49,6 +54,7 @@ void set_grad_peers(int64_t world, int64_t rank, std::vector<int64_t> ptrs, int6
   for (int i = 0; i < world; ++i) g_grad_peers.base[i] = reinterpret_cast<float*>(ptrs[i]);
 }
 void set_grad_push(bool on) { g_grad_peers.push = on ? 1 : 0; }
+int64_t grad_peers_world() { return g_grad_peers.world; }
 
 // optional fp8 side output: (q bytes, meta record, e5m2)
 inline b200::Fp8Out mk_fp8(const c10::optional<Tensor>& q, const c10::optional<Tensor>& meta, bool e5m2, int64_t numel) {
@@ -208,7 +214,8 @@ int64_t ln_bwd_workspace(int64_t M, int64_t H) { return b200::ln_bwd_workspace_f
 void layer_norm_bwd(Tensor dy, Tensor x, Tensor mean, Tensor rstd, Tensor gamma, Tensor dx, c10::optional<Tensor> dxd,
                     c10::optional<Tensor> dgamma, c10::optional<Tensor> dbeta, c10::optional<Tensor> dbias,
                     Tensor workspace, double p_drop, int64_t seed, int64_t drop_stream, int64_t in_stream,
-                    c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2, c10::optional<Tensor> keep_mask) {
+                    c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2, c10::optional<Tensor> keep_mask,
+                    bool deterministic) {
   check_ln_width(x.size(-1));
   check_bf16(dy, "dy"); check_bf16(x, "x"); check_bf16(dx, "dx");
   const int H = (int)x.size(-1), M = (int)(x.numel() / H);
@@ -225,7 +232,8 @@ void layer_norm_bwd(Tensor dy, Tensor x, Tensor mean, Tensor rstd, Tensor gamma,
   b200::layer_norm_bwd(dy.data_ptr(), x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
                        gamma.data_ptr<float>(), dx.data_ptr(), dxd_p, opt_f32(dgamma), opt_f32(dbeta), opt_f32(dbias),
                        workspace.data_ptr<float>(), M, H, mk_seed(seed), (unsigned)drop_stream,
-                       (unsigned)in_stream, (float)p_drop, mk_fp8(q8, meta8, e5m2, x.numel()), cur_stream(), km);
+                       (unsigned)in_stream, (float)p_drop, mk_fp8(q8, meta8, e5m2, x.numel()), cur_stream(), km,
+                       deterministic);
 }
 
 void gelu_fwd(Tensor x, Tensor y, c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2) {
@@ -235,20 +243,41 @@ void gelu_fwd(Tensor x, Tensor y, c10::optional<Tensor> q8, c10::optional<Tensor
   b200::gelu_fwd(x.data_ptr(), y.data_ptr(), x.numel(), mk_fp8(q8, meta8, e5m2, x.numel()), cur_stream());
 }
 void dgelu_bwd(Tensor dy, Tensor x, Tensor dx, c10::optional<Tensor> dbias, c10::optional<Tensor> q8,
-               c10::optional<Tensor> meta8, bool e5m2) {
+               c10::optional<Tensor> meta8, bool e5m2, bool deterministic) {
   check_bf16(dy, "dy"); check_bf16(x, "x"); check_bf16(dx, "dx");
   TORCH_CHECK(dy.dim() == 2 && dy.is_contiguous() && x.is_contiguous() && dx.is_contiguous() && dy.size(1) % 8 == 0,
               "dgelu_bwd: contiguous [M,N] with N % 8 == 0");
   c10::cuda::CUDAGuard guard(x.device());
-  b200::dgelu_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), opt_f32(dbias), (int)dy.size(0), (int)dy.size(1),
-                  mk_fp8(q8, meta8, e5m2, dy.numel()), cur_stream());
+  const int M = (int)dy.size(0), N = (int)dy.size(1);
+  Tensor ws;
+  if (deterministic && opt_f32(dbias) != nullptr) ws = f32_workspace(dy, b200::dgelu_det_workspace_floats(M, N));
+  b200::dgelu_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), opt_f32(dbias), M, N, mk_fp8(q8, meta8, e5m2, dy.numel()),
+                  cur_stream(), ws.defined() ? ws.data_ptr<float>() : nullptr);
 }
 
-void colsum(Tensor x, Tensor out) {
+void colsum(Tensor x, Tensor out, bool deterministic) {
   check_bf16(x, "x");
   TORCH_CHECK(x.dim() == 2 && out.scalar_type() == at::kFloat && out.numel() == x.size(1), "colsum shapes");
   c10::cuda::CUDAGuard guard(x.device());
-  b200::colsum_bf16(x.data_ptr(), (int)x.size(0), (int)x.size(1), (int)x.stride(0), out.data_ptr<float>(), cur_stream());
+  const int M = (int)x.size(0), N = (int)x.size(1);
+  if (deterministic) {
+    TORCH_CHECK(N % 8 == 0 && x.stride(0) % 8 == 0, "deterministic colsum: N and the row stride must be multiples of 8");
+    Tensor ws = f32_workspace(out, b200::colsum_det_workspace_floats(M, N));
+    b200::colsum_bf16_det(x.data_ptr(), M, N, (int)x.stride(0), out.data_ptr<float>(), ws.data_ptr<float>(), cur_stream());
+    return;
+  }
+  b200::colsum_bf16(x.data_ptr(), M, N, (int)x.stride(0), out.data_ptr<float>(), cur_stream());
+}
+
+// out[W] += part[rows, W] summed over the rows in row order (deterministic mode)
+void ordered_sum(Tensor part, Tensor out) {
+  TORCH_CHECK(part.is_cuda() && part.scalar_type() == at::kFloat && part.is_contiguous() && part.dim() >= 2,
+              "ordered_sum: contiguous fp32 part [rows, ...]");
+  TORCH_CHECK(out.scalar_type() == at::kFloat && out.is_contiguous() && out.numel() * part.size(0) == part.numel(),
+              "ordered_sum: out must be a contiguous fp32 tensor of one row of part");
+  c10::cuda::CUDAGuard guard(part.device());
+  b200::ordered_sum(part.data_ptr<float>(), (int)part.size(0), (int)out.numel(), nullptr, 1, out.data_ptr<float>(),
+                    cur_stream());
 }
 
 // pos_ids (optional int32 [M]): position of every token row (packed rows of an unpadded batch); else row % S
@@ -280,10 +309,26 @@ void embedding_fwd(Tensor ids, c10::optional<Tensor> seg, Tensor word, Tensor po
 }
 
 void embedding_bwd_scatter(Tensor de, Tensor ids, c10::optional<Tensor> seg, Tensor gword, Tensor gpos,
-                           c10::optional<Tensor> gtype, int64_t S, c10::optional<Tensor> pos_ids) {
+                           c10::optional<Tensor> gtype, int64_t S, c10::optional<Tensor> pos_ids, bool deterministic) {
   check_bf16(de, "de");
   const int H = (int)de.size(-1), M = (int)ids.numel();
   c10::cuda::CUDAGuard guard(de.device());
+  if (deterministic) {
+    TORCH_CHECK(H % 8 == 0 && de.is_contiguous(), "deterministic embedding backward: contiguous de with H % 8 == 0");
+    TORCH_CHECK(S > 0, "deterministic embedding backward: S must be positive");
+    const int chunk = std::min(M, b200::embedding_det_chunk_rows());   // rows sorted at a time
+    int64_t rows = std::max(gword.size(0), gpos.size(0));
+    if (gtype.has_value() && gtype->defined()) rows = std::max(rows, gtype->size(0));
+    TORCH_CHECK(rows * (int64_t)chunk < (int64_t(1) << 32), "deterministic embedding backward: table rows x ", chunk,
+                " must stay below 2^32");
+    Tensor sort_ws = at::empty({std::max(chunk, 1)}, ids.options().dtype(at::kInt));
+    Tensor sum_ws = f32_workspace(gword, (int64_t)chunk * H);
+    b200::embedding_bwd_det(de.data_ptr(), ids.data_ptr<int>(),
+                            seg.has_value() && seg->defined() ? seg->data_ptr<int>() : nullptr, gword.data_ptr<float>(),
+                            gpos.data_ptr<float>(), opt_f32(gtype), M, (int)S, H, opt_pos_ids(pos_ids, ids),
+                            reinterpret_cast<unsigned*>(sort_ws.data_ptr<int>()), sum_ws.data_ptr<float>(), cur_stream());
+    return;
+  }
   b200::embedding_bwd_scatter(de.data_ptr(), ids.data_ptr<int>(),
                               seg.has_value() && seg->defined() ? seg->data_ptr<int>() : nullptr,
                               gword.data_ptr<float>(), gpos.data_ptr<float>(), opt_f32(gtype), M, (int)S, H,
@@ -353,12 +398,15 @@ void scatter_rows(Tensor src, Tensor idx, Tensor dst) {
   b200::scatter_rows(src.data_ptr(), idx.data_ptr<int>(), dst.data_ptr(), (int)idx.numel(), (int)src.size(-1), cur_stream());
 }
 
-void softmax_ce(Tensor logits, Tensor targets, Tensor count, double grad_scale, Tensor loss_out) {
+void softmax_ce(Tensor logits, Tensor targets, Tensor count, double grad_scale, Tensor loss_out, bool deterministic) {
   check_bf16(logits, "logits");
   TORCH_CHECK(logits.dim() == 2 && logits.size(1) % 8 == 0 && logits.stride(0) % 8 == 0, "logits: [R,V], V%8==0");
   c10::cuda::CUDAGuard guard(logits.device());
+  Tensor rows;
+  if (deterministic) rows = f32_workspace(loss_out, logits.size(0));
   b200::softmax_ce(logits.data_ptr(), (int)logits.stride(0), targets.data_ptr<int>(), count.data_ptr<int>(),
-                   (float)grad_scale, loss_out.data_ptr<float>(), (int)logits.size(0), (int)logits.size(1), cur_stream());
+                   (float)grad_scale, loss_out.data_ptr<float>(), (int)logits.size(0), (int)logits.size(1), cur_stream(),
+                   deterministic ? rows.data_ptr<float>() : nullptr);
 }
 
 inline int dtype_code(const Tensor& t) {
@@ -370,11 +418,14 @@ inline int dtype_code(const Tensor& t) {
 }
 
 void mt_l2norm(int64_t dtype, Tensor ptrs, Tensor chunk_tensor, Tensor chunk_start, Tensor chunk_len,
-               c10::optional<Tensor> per_tensor_sq, Tensor total_sq) {
+               c10::optional<Tensor> per_tensor_sq, Tensor total_sq, bool deterministic) {
   c10::cuda::CUDAGuard guard(ptrs.device());
+  Tensor ws;
+  if (deterministic) ws = f32_workspace(total_sq, chunk_tensor.numel());
   b200::mt_l2norm((int)dtype, (const long long*)ptrs.data_ptr<int64_t>(), chunk_tensor.data_ptr<int>(),
                   (const long long*)chunk_start.data_ptr<int64_t>(), chunk_len.data_ptr<int>(),
-                  (int)chunk_tensor.numel(), opt_f32(per_tensor_sq), total_sq.data_ptr<float>(), cur_stream());
+                  (int)chunk_tensor.numel(), opt_f32(per_tensor_sq), total_sq.data_ptr<float>(), cur_stream(),
+                  deterministic ? ws.data_ptr<float>() : nullptr, (int)ptrs.numel());
 }
 void mt_scale(int64_t in_dtype, int64_t out_dtype, Tensor in_ptrs, Tensor out_ptrs, Tensor chunk_tensor,
               Tensor chunk_start, Tensor chunk_len, c10::optional<Tensor> scale_dev, double scale_host, Tensor overflow) {
@@ -384,10 +435,14 @@ void mt_scale(int64_t in_dtype, int64_t out_dtype, Tensor in_ptrs, Tensor out_pt
                  (const long long*)chunk_start.data_ptr<int64_t>(), chunk_len.data_ptr<int>(), (int)chunk_tensor.numel(),
                  opt_f32(scale_dev), (float)scale_host, overflow.data_ptr<int>(), cur_stream());
 }
-void flat_sumsq(Tensor g, c10::optional<Tensor> inv_scale, Tensor stats, c10::optional<Tensor> found_inf) {
+void flat_sumsq(Tensor g, c10::optional<Tensor> inv_scale, Tensor stats, c10::optional<Tensor> found_inf,
+                bool deterministic) {
   c10::cuda::CUDAGuard guard(g.device());
   TORCH_CHECK(g.numel() % 4 == 0, "arena size must be a multiple of 4");
-  b200::flat_sumsq(g.data_ptr<float>(), g.numel(), opt_f32(inv_scale), stats.data_ptr<float>(), opt_f32(found_inf), cur_stream());
+  Tensor ws;
+  if (deterministic) ws = f32_workspace(stats, b200::flat_sumsq_det_blocks());
+  b200::flat_sumsq(g.data_ptr<float>(), g.numel(), opt_f32(inv_scale), stats.data_ptr<float>(), opt_f32(found_inf), cur_stream(),
+                   deterministic ? ws.data_ptr<float>() : nullptr);
 }
 void flat_unscale(Tensor g, Tensor inv_scale, Tensor found_inf) {
   c10::cuda::CUDAGuard guard(g.device());
@@ -398,15 +453,17 @@ void arena_lamb(Tensor g, Tensor p, Tensor m, Tensor v, c10::optional<Tensor> sh
                 Tensor chunk_start, Tensor chunk_len, Tensor decay_flag, Tensor stats, Tensor norms,
                 c10::optional<Tensor> inv_scale, c10::optional<Tensor> found_inf, double lr, double beta1, double beta2,
                 double eps, double weight_decay, int64_t step, bool bias_correction, bool grad_averaging,
-                double max_grad_norm, bool adam_w_mode, bool use_nvlamb) {
+                double max_grad_norm, bool adam_w_mode, bool use_nvlamb, bool deterministic) {
   c10::cuda::CUDAGuard guard(g.device());
+  Tensor ws;
+  if (deterministic) ws = f32_workspace(norms, 2 * chunk_tensor.numel());
   b200::arena_lamb(g.data_ptr<float>(), p.data_ptr<float>(), m.data_ptr<float>(), v.data_ptr<float>(),
                    shadow.has_value() && shadow->defined() ? shadow->data_ptr() : nullptr, chunk_tensor.data_ptr<int>(),
                    (const long long*)chunk_start.data_ptr<int64_t>(), chunk_len.data_ptr<int>(), (int)chunk_tensor.numel(),
                    decay_flag.data_ptr<int>(), (int)decay_flag.numel(), stats.data_ptr<float>(), norms.data_ptr<float>(),
                    opt_f32(inv_scale), opt_f32(found_inf), (float)lr, (float)beta1, (float)beta2, (float)eps,
                    (float)weight_decay, (int)step, bias_correction, grad_averaging, (float)max_grad_norm, adam_w_mode,
-                   use_nvlamb, cur_stream());
+                   use_nvlamb, cur_stream(), deterministic ? ws.data_ptr<float>() : nullptr);
 }
 void arena_adam(Tensor g, Tensor p, Tensor m, Tensor v, c10::optional<Tensor> shadow, Tensor chunk_tensor,
                 Tensor chunk_start, Tensor chunk_len, Tensor decay_flag, c10::optional<Tensor> inv_scale,
@@ -478,19 +535,20 @@ void attention_fwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor
 void attention_bwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor dctx, Tensor lse, Tensor dqkv,
                    Tensor delta_ws, c10::optional<Tensor> dq_acc, int64_t heads, double scale, double p_drop, int64_t seed,
                    int64_t stream_id, c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2,
-                   c10::optional<Tensor> cu_seqlens, int64_t S) {
+                   c10::optional<Tensor> cu_seqlens, int64_t S, bool deterministic) {
   const AttnShape a = check_attention(qkv, seqlens, lse, heads, cu_seqlens, S, q8.has_value() && q8->defined());
   check_bf16(qkv, "qkv"); check_bf16(ctx, "ctx"); check_bf16(dctx, "dctx"); check_bf16(dqkv, "dqkv");
   TORCH_CHECK(qkv.is_contiguous() && ctx.is_contiguous() && dctx.is_contiguous() && dqkv.is_contiguous(), "attention_bwd needs contiguous tensors");
   TORCH_CHECK(ctx.numel() == a.rows * a.H && dctx.numel() == ctx.numel() && dqkv.numel() == qkv.numel(),
               "attention_bwd: ctx / dctx [rows, H] and dqkv like qkv");
-  TORCH_CHECK(!dq_acc.has_value() || !dq_acc->defined() || dq_acc->numel() >= a.rows * a.H,
-              "attention_bwd: dq_acc must hold [rows, H] floats");
+  const int slices = b200::attention_dq_slices(a.S, deterministic);
+  TORCH_CHECK(!dq_acc.has_value() || !dq_acc->defined() || dq_acc->numel() >= slices * a.rows * a.H,
+              "attention_bwd: dq_acc must hold ", slices, " x [rows, H] floats");
   c10::cuda::CUDAGuard guard(qkv.device());
   b200::attention_bwd(qkv.data_ptr(), a.seqlens, ctx.data_ptr(), dctx.data_ptr(), lse.data_ptr<float>(),
                       dqkv.data_ptr(), delta_ws.data_ptr<float>(), opt_f32(dq_acc), a.B, a.S, (int)heads, a.H / (int)heads,
                       (float)scale, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
-                      mk_fp8(q8, meta8, e5m2, dqkv.numel()), cur_stream(), a.cu, a.rows);
+                      mk_fp8(q8, meta8, e5m2, dqkv.numel()), cur_stream(), a.cu, a.rows, deterministic);
 }
 
 void fused_allreduce_lamb(int64_t rank, int64_t world, bool use_multicast, std::vector<int64_t> grad_ptrs,
@@ -536,7 +594,7 @@ void fused_allreduce_lamb(int64_t rank, int64_t world, bool use_multicast, std::
 }
 
 void nsp_head(Tensor pooled, Tensor w, Tensor bias, Tensor labels, double grad_scale, Tensor loss_out, Tensor dz, Tensor dw,
-              Tensor db) {
+              Tensor db, bool deterministic) {
   check_bf16(pooled, "pooled"); check_bf16(w, "w"); check_bf16(dz, "dz");
   TORCH_CHECK(pooled.dim() == 2 && pooled.is_contiguous() && dz.is_contiguous() && dz.sizes() == pooled.sizes(), "nsp_head: pooled/dz");
   const int64_t B = pooled.size(0), H = pooled.size(1);
@@ -548,7 +606,7 @@ void nsp_head(Tensor pooled, Tensor w, Tensor bias, Tensor labels, double grad_s
   c10::cuda::CUDAGuard guard(pooled.device());
   b200::nsp_head(pooled.data_ptr(), w.data_ptr(), bias.data_ptr<float>(), reinterpret_cast<const long long*>(labels.data_ptr<int64_t>()), (int)B, (int)H,
                  (float)grad_scale, loss_out.data_ptr<float>(), dz.data_ptr(), dw.data_ptr<float>(), db.data_ptr<float>(),
-                 cur_stream());
+                 cur_stream(), deterministic ? f32_workspace(dw, B * (3 + 2 * H)).data_ptr<float>() : nullptr);
 }
 
 void peer_allreduce(int64_t rank, int64_t world, bool use_multicast, std::vector<int64_t> buf_ptrs,
@@ -610,14 +668,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("set_seed_step", &set_seed_step);
   m.def("set_grad_peers", &set_grad_peers);
   m.def("set_grad_push", &set_grad_push);
+  m.def("grad_peers_world", &grad_peers_world);
   m.def("peer_allreduce", &peer_allreduce);
   m.def("fp8_quantize", &fp8_quantize);
   m.def("fp8_amax", &fp8_amax);
   m.def("fp8_update", &fp8_update);
   m.def("layer_norm_fwd", &layer_norm_fwd);
-  m.def("layer_norm_bwd", &layer_norm_bwd);
+  m.def("layer_norm_bwd", &layer_norm_bwd, pybind11::arg("dy"), pybind11::arg("x"), pybind11::arg("mean"),
+        pybind11::arg("rstd"), pybind11::arg("gamma"), pybind11::arg("dx"), pybind11::arg("dxd"),
+        pybind11::arg("dgamma"), pybind11::arg("dbeta"), pybind11::arg("dbias"), pybind11::arg("workspace"),
+        pybind11::arg("p_drop"), pybind11::arg("seed"), pybind11::arg("drop_stream"), pybind11::arg("in_stream"),
+        pybind11::arg("q8"), pybind11::arg("meta8"), pybind11::arg("e5m2"), pybind11::arg("keep_mask"),
+        pybind11::arg("deterministic") = false);
   m.def("ln_bwd_workspace", &ln_bwd_workspace);
   m.def("colsum", &colsum);
+  m.def("ordered_sum", &ordered_sum);
   m.def("gelu_fwd", &gelu_fwd);
   m.def("dgelu_bwd", &dgelu_bwd);
   m.def("embedding_fwd", &embedding_fwd);
@@ -636,6 +701,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("arena_lamb", &arena_lamb);
   m.def("arena_adam", &arena_adam);
   m.def("attention_fwd", &attention_fwd);
-  m.def("attention_bwd", &attention_bwd);
+  m.def("attention_bwd", &attention_bwd, pybind11::arg("qkv"), pybind11::arg("seqlens"), pybind11::arg("ctx"),
+        pybind11::arg("dctx"), pybind11::arg("lse"), pybind11::arg("dqkv"), pybind11::arg("delta_ws"),
+        pybind11::arg("dq_acc"), pybind11::arg("heads"), pybind11::arg("scale"), pybind11::arg("p_drop"),
+        pybind11::arg("seed"), pybind11::arg("stream_id"), pybind11::arg("q8"), pybind11::arg("meta8"),
+        pybind11::arg("e5m2"), pybind11::arg("cu_seqlens"), pybind11::arg("S"),
+        pybind11::arg("deterministic") = false);
   m.def("fused_allreduce_lamb", &fused_allreduce_lamb);
 }

@@ -14,12 +14,29 @@ int ln_bwd_workspace_floats(int M, int H);
 void layer_norm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const float* gamma, void* dx,
                     void* dxd, float* dgamma, float* dbeta, float* dbias, float* workspace, int M, int H,
                     Seed seed, unsigned int drop_stream, unsigned int in_stream, float p_drop, Fp8Out f8,
-                    cudaStream_t st, const uint8_t* keep_mask = nullptr);
+                    cudaStream_t st, const uint8_t* keep_mask = nullptr, bool deterministic = false);
 void gelu_fwd(const void* x, void* y, long long n, Fp8Out f8, cudaStream_t st);
-void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int N, Fp8Out f8, cudaStream_t st);
+// dbias_ws (deterministic mode, dgelu_det_workspace_floats(M, N) floats): the blocks' fp32 column sums are stored there
+// and added to dbias in order
+int dgelu_det_workspace_floats(int M, int N);
+void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int N, Fp8Out f8, cudaStream_t st,
+               float* dbias_ws = nullptr);
 // keep bits ([n_elems / 8] bytes, n_elems % 32 == 0) of the dropout stream (seed, stream): see dropout_mask_kernel
 void dropout_mask(void* out, long long n_elems, Seed seed, unsigned int stream, float p_drop, cudaStream_t st);
 void colsum_bf16(const void* x, int M, int N, int ld, float* out, cudaStream_t st);
+
+// Deterministic mode: fixed-order forms of the reductions (no atomics; the order of every sum depends on the shapes only).
+// out[s * W + w] += sum over the rows r of segment s, in a fixed order, of part[r * W + w]; row_seg (ascending, int32
+// [rows]) assigns rows to the nseg segments, or is null for one segment of every row
+void ordered_sum(const float* part, int rows, int W, const int* row_seg, int nseg, float* out, cudaStream_t st);
+// colsum_bf16 through a workspace of colsum_det_workspace_floats(M, N) floats
+int colsum_det_workspace_floats(int M, int N);
+void colsum_bf16_det(const void* x, int M, int N, int ld, float* out, float* ws, cudaStream_t st);
+// embedding_bwd_scatter by sorting the rows by table row, embedding_det_chunk_rows() rows at a time (chunks added in
+// order; table rows * chunk < 2^32); workspaces: sort_ws [chunk], sum_ws [chunk, H].  A null seg means segment 0.
+int embedding_det_chunk_rows();
+void embedding_bwd_det(const void* de, const int* ids, const int* seg, float* gword, float* gpos, float* gtype,
+                       int M, int S, int H, const int* pos_ids, unsigned* sort_ws, float* sum_ws, cudaStream_t st);
 void embedding_fwd(const int* ids, const int* seg, const void* word, const void* pos, const void* type,
                    const float* gamma, const float* beta, void* e_out, void* y, float* mean, float* rstd, int M, int S,
                    int H, float eps, Seed seed, unsigned int stream, float p_drop, cudaStream_t st,
@@ -38,22 +55,28 @@ void gather_rows(const void* src, const int* idx, void* dst, int n, int H, cudaS
 void scatter_rows(const void* src, const int* idx, void* dst, int n, int H, cudaStream_t st);
 
 // loss.cu
+// loss_rows (float [R], deterministic mode): per-row terms, then added to loss_out in row order
 void softmax_ce(void* logits, int ld, const int* targets, const int* count, float grad_scale, float* loss_out, int R,
-                int V, cudaStream_t st);
+                int V, cudaStream_t st, float* loss_rows = nullptr);
 
 // optim.cu   (dtype codes: 0 = fp32, 1 = bf16, 2 = fp16)
 void mt_l2norm(int dtype, const long long* ptrs, const int* chunk_tensor, const long long* chunk_start,
-               const int* chunk_len, int nchunks, float* per_tensor_sq, float* total_sq, cudaStream_t st);
+               const int* chunk_len, int nchunks, float* per_tensor_sq, float* total_sq, cudaStream_t st,
+               float* chunk_ws = nullptr, int ntensors = 0);   // chunk_ws [nchunks]: deterministic mode
 void mt_scale(int in_dtype, int out_dtype, const long long* in_ptrs, const long long* out_ptrs,
               const int* chunk_tensor, const long long* chunk_start, const int* chunk_len, int nchunks,
               const float* scale_dev, float scale_host, int* overflow, cudaStream_t st);
-void flat_sumsq(const float* g, long long n, const float* inv_scale, float* stats, float* found_inf, cudaStream_t st);
+// block_ws [flat_sumsq_det_blocks()]: deterministic mode
+int flat_sumsq_det_blocks();
+void flat_sumsq(const float* g, long long n, const float* inv_scale, float* stats, float* found_inf, cudaStream_t st,
+                float* block_ws = nullptr);
 void flat_unscale(float* g, long long n, const float* inv_scale, float* found_inf, cudaStream_t st);
 void arena_lamb(float* g, float* p, float* m, float* v, void* shadow, const int* chunk_tensor,
                 const long long* chunk_start, const int* chunk_len, int nchunks, const int* decay_flag,
                 int ntensors, float* stats, float* norms, const float* inv_scale, const float* found_inf,
                 float lr, float beta1, float beta2, float eps, float weight_decay, int step, int bias_correction,
-                int grad_averaging, float max_grad_norm, int adam_w_mode, int use_nvlamb, cudaStream_t st);
+                int grad_averaging, float max_grad_norm, int adam_w_mode, int use_nvlamb, cudaStream_t st,
+                float* chunk_ws = nullptr);   // chunk_ws [2 * nchunks]: deterministic mode
 void arena_adam(float* g, float* p, float* m, float* v, void* shadow, const int* chunk_tensor,
                 const long long* chunk_start, const int* chunk_len, int nchunks, const int* decay_flag,
                 const float* inv_scale, const float* found_inf, float lr, float beta1, float beta2, float eps,
@@ -70,7 +93,9 @@ void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, i
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
                    Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
-                   const int* cu_seqlens = nullptr, long long T = 0);
+                   const int* cu_seqlens = nullptr, long long T = 0, bool deterministic = false);
+// deterministic attention_bwd: dq_acc holds attention_dq_slices(S) slices of [rows, H]
+inline int attention_dq_slices(int S, bool deterministic) { return deterministic && S > 128 ? (S + 127) / 128 : 1; }
 
 // comm.cu -- fused peer-memory all-reduce + partitioned LAMB (one cooperative kernel per step)
 struct FusedLambLaunch {
@@ -105,7 +130,8 @@ void peer_allreduce(const PeerAllreduceLaunch& L, cudaStream_t st);
 
 // loss.cu: NSP classifier + CE + backward in one launch
 void nsp_head(const void* pooled_bf16, const void* w_bf16, const float* bias, const long long* labels, int B, int H,
-              float grad_scale, float* loss_out, void* dz_bf16, float* dw, float* db, cudaStream_t st);
+              float grad_scale, float* loss_out, void* dz_bf16, float* dw, float* db, cudaStream_t st,
+              float* rows_ws = nullptr);   // rows_ws [B * (3 + 2 H)]: deterministic mode
 
 // fp8.cu: per-tensor scaled fp8 operand preparation; meta records are {amax, scale, inv_scale, _}
 void fp8_quantize(const void* x_bf16, void* q, long long n, float* meta, bool e5m2, cudaStream_t st);

@@ -10,9 +10,12 @@ namespace b200 {
 
 constexpr int CE_THREADS = 256;
 
-__global__ void __launch_bounds__(CE_THREADS)
-softmax_ce_kernel(__nv_bfloat16* __restrict__ logits, int ld, const int* __restrict__ targets,
-                  const int* __restrict__ count, float grad_scale, float* __restrict__ loss_out, int V) {
+// ROWS (deterministic mode): loss_out[r] receives row r's term (0 for an ignored row) instead of an atomic add into
+// loss_out[0]; ordered_sum then adds the rows in order.
+template <bool ROWS>
+__device__ __forceinline__ void softmax_ce_body(__nv_bfloat16* __restrict__ logits, int ld, const int* __restrict__ targets,
+                                                const int* __restrict__ count, float grad_scale,
+                                                float* __restrict__ loss_out, int V) {
   __shared__ float sm[32];
   __shared__ float s_max, s_sum;
   const int r = blockIdx.x;
@@ -21,6 +24,7 @@ softmax_ce_kernel(__nv_bfloat16* __restrict__ logits, int ld, const int* __restr
   const int nvec = V >> 3;  // V % 8 == 0
   uint4* row4 = reinterpret_cast<uint4*>(row);
   if (tgt < 0) {  // ignored position: zero gradient row
+    if constexpr (ROWS) if (threadIdx.x == 0) loss_out[r] = 0.f;
     for (int i = threadIdx.x; i < nvec; i += CE_THREADS) row4[i] = make_uint4(0, 0, 0, 0);
     return;
   }
@@ -72,7 +76,8 @@ softmax_ce_kernel(__nv_bfloat16* __restrict__ logits, int ld, const int* __restr
   const float gs = grad_scale / cnt;
   if (threadIdx.x == 0) {
     const float lt = __bfloat162float(row[tgt]);
-    atomicAdd(loss_out, (logf(s_sum) + gmax - lt) / cnt);
+    if constexpr (ROWS) loss_out[r] = (logf(s_sum) + gmax - lt) / cnt;
+    else atomicAdd(loss_out, (logf(s_sum) + gmax - lt) / cnt);
   }
   __syncthreads();  // the target logit was read before anyone overwrites it
   // pass 2: gradient in place
@@ -95,9 +100,27 @@ softmax_ce_kernel(__nv_bfloat16* __restrict__ logits, int ld, const int* __restr
   }
 }
 
+__global__ void __launch_bounds__(CE_THREADS)
+softmax_ce_kernel(__nv_bfloat16* __restrict__ logits, int ld, const int* __restrict__ targets,
+                  const int* __restrict__ count, float grad_scale, float* __restrict__ loss_out, int V) {
+  softmax_ce_body<false>(logits, ld, targets, count, grad_scale, loss_out, V);
+}
+
+__global__ void __launch_bounds__(CE_THREADS)
+softmax_ce_rows_kernel(__nv_bfloat16* __restrict__ logits, int ld, const int* __restrict__ targets,
+                       const int* __restrict__ count, float grad_scale, float* __restrict__ loss_rows, int V) {
+  softmax_ce_body<true>(logits, ld, targets, count, grad_scale, loss_rows, V);
+}
+
 void softmax_ce(void* logits, int ld, const int* targets, const int* count, float grad_scale, float* loss_out, int R,
-                int V, cudaStream_t st) {
-  if (R > 0) softmax_ce_kernel<<<R, CE_THREADS, 0, st>>>((__nv_bfloat16*)logits, ld, targets, count, grad_scale, loss_out, V);
+                int V, cudaStream_t st, float* loss_rows) {
+  if (R <= 0) return;
+  if (loss_rows == nullptr) {
+    softmax_ce_kernel<<<R, CE_THREADS, 0, st>>>((__nv_bfloat16*)logits, ld, targets, count, grad_scale, loss_out, V);
+    return;
+  }
+  softmax_ce_rows_kernel<<<R, CE_THREADS, 0, st>>>((__nv_bfloat16*)logits, ld, targets, count, grad_scale, loss_rows, V);
+  ordered_sum(loss_rows, R, 1, nullptr, 1, loss_out, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -106,10 +129,13 @@ void softmax_ce(void* logits, int ld, const int* targets, const int* count, floa
 // atomics and the gradient of the pooler pre-activation  dz = (dlogits . W) * (1 - pooled^2)  (tanh' folded in).
 // One block per sequence; pooled is the bf16 output of the pooler GEMM's bias+tanh epilogue.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128)
-nsp_head_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
-                const long long* __restrict__ labels, int B, int H, float grad_scale, float* __restrict__ loss_out,
-                __nv_bfloat16* __restrict__ dz, float* __restrict__ dw, float* __restrict__ db) {
+// ROWS (deterministic mode): sequence b stores its loss term, db and dW contributions to loss_out[b], db[2 b + k] and
+// dw[2 H b + k H + i] (zeros when it contributes nothing) for ordered_sum, instead of atomics.
+template <bool ROWS>
+__device__ __forceinline__ void nsp_head_body(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w,
+                                              const float* __restrict__ bias, const long long* __restrict__ labels, int B,
+                                              int H, float grad_scale, float* __restrict__ loss_out,
+                                              __nv_bfloat16* __restrict__ dz, float* __restrict__ dw, float* __restrict__ db) {
   __shared__ float sm[32];
   __shared__ float s_bc[3];
   const int b = blockIdx.x;
@@ -134,16 +160,23 @@ nsp_head_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* _
   };
   const float l0 = block_sum(a0) + bias[0], l1 = block_sum(a1) + bias[1];
   float d0 = 0.f, d1 = 0.f;
+  if constexpr (ROWS) {
+    if (threadIdx.x == 0) loss_out[b] = 0.f;
+    loss_out += b; db += 2 * b; dw += (size_t)2 * H * b;
+  }
   if (y >= 0 && n_valid > 0) {
     const float m = fmaxf(l0, l1);
     const float lse = m + logf(expf(l0 - m) + expf(l1 - m));
     const float p0 = expf(l0 - lse), p1 = expf(l1 - lse);
     const float inv = 1.f / (float)n_valid;
-    if (threadIdx.x == 0) atomicAdd(loss_out, (lse - (y == 0 ? l0 : l1)) * inv);
+    if constexpr (ROWS) { if (threadIdx.x == 0) *loss_out = (lse - (y == 0 ? l0 : l1)) * inv; }
+    else if (threadIdx.x == 0) atomicAdd(loss_out, (lse - (y == 0 ? l0 : l1)) * inv);
     d0 = (p0 - (y == 0 ? 1.f : 0.f)) * inv * grad_scale;
     d1 = (p1 - (y == 1 ? 1.f : 0.f)) * inv * grad_scale;
   }
-  if (threadIdx.x == 0 && (d0 != 0.f || d1 != 0.f)) {
+  if constexpr (ROWS) {
+    if (threadIdx.x == 0) { db[0] = d0; db[1] = d1; }
+  } else if (threadIdx.x == 0 && (d0 != 0.f || d1 != 0.f)) {
     atomicAdd(db, d0);
     atomicAdd(db + 1, d1);
   }
@@ -151,18 +184,48 @@ nsp_head_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* _
     const float xv = __bfloat162float(x[i]);
     const float g = d0 * __bfloat162float(w[i]) + d1 * __bfloat162float(w[H + i]);
     dz[(size_t)b * H + i] = __float2bfloat16(g * (1.f - xv * xv));
-    if (d0 != 0.f || d1 != 0.f) {
+    if constexpr (ROWS) {
+      const bool live = d0 != 0.f || d1 != 0.f;
+      dw[i] = live ? d0 * xv : 0.f;
+      dw[H + i] = live ? d1 * xv : 0.f;
+    } else if (d0 != 0.f || d1 != 0.f) {
       atomicAdd(dw + i, d0 * xv);
       atomicAdd(dw + H + i, d1 * xv);
     }
   }
 }
 
+__global__ void __launch_bounds__(128)
+nsp_head_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
+                const long long* __restrict__ labels, int B, int H, float grad_scale, float* __restrict__ loss_out,
+                __nv_bfloat16* __restrict__ dz, float* __restrict__ dw, float* __restrict__ db) {
+  nsp_head_body<false>(pooled, w, bias, labels, B, H, grad_scale, loss_out, dz, dw, db);
+}
+
+__global__ void __launch_bounds__(128)
+nsp_head_rows_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w,
+                     const float* __restrict__ bias, const long long* __restrict__ labels, int B, int H, float grad_scale,
+                     float* __restrict__ loss_rows, __nv_bfloat16* __restrict__ dz, float* __restrict__ dw_rows,
+                     float* __restrict__ db_rows) {
+  nsp_head_body<true>(pooled, w, bias, labels, B, H, grad_scale, loss_rows, dz, dw_rows, db_rows);
+}
+
 void nsp_head(const void* pooled, const void* w, const float* bias, const long long* labels, int B, int H, float grad_scale,
-              float* loss_out, void* dz, float* dw, float* db, cudaStream_t st) {
-  if (B > 0)
+              float* loss_out, void* dz, float* dw, float* db, cudaStream_t st, float* rows_ws) {
+  if (B <= 0) return;
+  if (rows_ws == nullptr) {
     nsp_head_kernel<<<B, 128, 0, st>>>((const __nv_bfloat16*)pooled, (const __nv_bfloat16*)w, bias, labels, B, H, grad_scale,
                                        loss_out, (__nv_bfloat16*)dz, dw, db);
+    return;
+  }
+  float* loss_rows = rows_ws;                 // [B], then db [B, 2], then dW [B, 2, H]
+  float* db_rows = rows_ws + B;
+  float* dw_rows = rows_ws + 3 * B;
+  nsp_head_rows_kernel<<<B, 128, 0, st>>>((const __nv_bfloat16*)pooled, (const __nv_bfloat16*)w, bias, labels, B, H,
+                                          grad_scale, loss_rows, (__nv_bfloat16*)dz, dw_rows, db_rows);
+  ordered_sum(loss_rows, B, 1, nullptr, 1, loss_out, st);
+  ordered_sum(db_rows, B, 2, nullptr, 1, db, st);
+  ordered_sum(dw_rows, B, 2 * H, nullptr, 1, dw, st);
 }
 
 }  // namespace b200

@@ -472,10 +472,12 @@ __global__ void __launch_bounds__(256) gelu_fwd_kernel(const __nv_bfloat16* __re
   if (f8.q) fp8_amax_commit(f8, amax);
 }
 
-// dx[m][n] = dy[m][n] * gelu'(x[m][n]);  dbias[n] += sum_m dx[m][n]
-__global__ void __launch_bounds__(256)
-dgelu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ dx,
-                 float* __restrict__ dbias, int M, int N, const Fp8Out f8) {
+// dx[m][n] = dy[m][n] * gelu'(x[m][n]);  dbias[n] += sum_m dx[m][n] (the fp32 products, before the bf16 rounding)
+// PART (deterministic mode): block (x, y) stores its column sums to dbias[y * N + col] for ordered_sum instead
+template <bool PART>
+__device__ __forceinline__ void dgelu_bwd_body(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                               __nv_bfloat16* __restrict__ dx, float* __restrict__ dbias, int M, int N,
+                                               const Fp8Out& f8) {
   const int cg = threadIdx.x & 31, rl = threadIdx.x >> 5;
   const int col = blockIdx.x * 256 + cg * 8;
   const float qscale = f8.q ? f8.meta[1] : 0.f;
@@ -523,7 +525,20 @@ dgelu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __re
   float sum = 0.f;
 #pragma unroll
   for (int r = 0; r < 8; ++r) sum += sm[r][c];
-  if (blockIdx.x * 256 + c < N) atomicAdd(dbias + blockIdx.x * 256 + c, sum);
+  if constexpr (PART) { if (blockIdx.x * 256 + c < N) dbias[(size_t)blockIdx.y * N + blockIdx.x * 256 + c] = sum; }
+  else if (blockIdx.x * 256 + c < N) atomicAdd(dbias + blockIdx.x * 256 + c, sum);
+}
+
+__global__ void __launch_bounds__(256)
+dgelu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ dx,
+                 float* __restrict__ dbias, int M, int N, const Fp8Out f8) {
+  dgelu_bwd_body<false>(dy, x, dx, dbias, M, N, f8);
+}
+
+__global__ void __launch_bounds__(256)
+dgelu_bwd_part_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                      __nv_bfloat16* __restrict__ dx, float* __restrict__ dbias_part, int M, int N, const Fp8Out f8) {
+  dgelu_bwd_body<true>(dy, x, dx, dbias_part, M, N, f8);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -662,6 +677,167 @@ embed_bwd_postype_kernel(const __nv_bfloat16* __restrict__ de, const int* __rest
     atomicAdd(gtype + blockIdx.x * 256 + c, t0);
     atomicAdd(gtype + H + blockIdx.x * 256 + c, t1);
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Deterministic mode (ops.api.deterministic()): fixed-order forms of the reductions above.  None of these kernels
+// waits on another CTA; the order of every floating-point sum depends only on the shapes.
+// ------------------------------------------------------------------------------------------------
+constexpr int ORD_THREADS = 256;
+
+// out[s * W + w] += sum over the rows r of segment s of part[r * W + w].  A block owns CW (a power of two <= 32)
+// columns; its R = 256 / CW row lanes sum rows lo + j, lo + j + R, ... each, and a fixed binary tree combines the
+// lanes.  Segment s is every row when row_seg is null (one segment), else the rows whose row_seg (ascending) is s.
+__global__ void __launch_bounds__(ORD_THREADS)
+ordered_sum_kernel(const float* __restrict__ part, int rows, int W, int CW, const int* __restrict__ row_seg,
+                   float* __restrict__ out) {
+  const int s = blockIdx.y;
+  int lo = 0, hi = rows;
+  if (row_seg != nullptr) {
+    auto lower = [&](int v) {
+      int a = 0, b = rows;
+      while (a < b) { const int m = (a + b) >> 1; if (row_seg[m] < v) a = m + 1; else b = m; }
+      return a;
+    };
+    lo = lower(s);
+    hi = lower(s + 1);
+  }
+  const int cl = threadIdx.x & (CW - 1), rl = threadIdx.x / CW, R = ORD_THREADS / CW;
+  const int w = blockIdx.x * CW + cl;
+  float acc = 0.f;
+  if (w < W) {
+#pragma unroll 4
+    for (int r = lo + rl; r < hi; r += R) acc += part[(size_t)r * W + w];
+  }
+  __shared__ float sm[ORD_THREADS];
+  sm[threadIdx.x] = acc;
+  __syncthreads();
+  for (int half = R >> 1; half > 0; half >>= 1) {
+    if (rl < half) sm[threadIdx.x] += sm[threadIdx.x + half * CW];
+    __syncthreads();
+  }
+  if (rl == 0 && w < W) out[(size_t)s * W + w] += sm[cl];
+}
+
+// colsum_bf16_kernel with the block's column sums stored to part[blockIdx.y][N] instead of added to the output
+__global__ void __launch_bounds__(256) colsum_bf16_part_kernel(const __nv_bfloat16* __restrict__ x, int M, int N, int ld,
+                                                              float* __restrict__ part) {
+  const int cg = threadIdx.x & 31, rl = threadIdx.x >> 5;
+  const int col = blockIdx.x * 256 + cg * 8;
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (col < N) {
+    for (int row = blockIdx.y * 8 + rl; row < M; row += gridDim.y * 8) {
+      float f[8];
+      unpack8(*reinterpret_cast<const uint4*>(x + (size_t)row * ld + col), f);
+#pragma unroll
+      for (int t = 0; t < 8; ++t) acc[t] += f[t];
+    }
+  }
+  __shared__ float sm[8][256];
+#pragma unroll
+  for (int t = 0; t < 8; ++t) sm[rl][cg * 8 + t] = acc[t];
+  __syncthreads();
+  const int c = threadIdx.x;
+  float s = 0.f;
+#pragma unroll
+  for (int r = 0; r < 8; ++r) s += sm[r][c];
+  if (blockIdx.x * 256 + c < N) part[(size_t)blockIdx.y * N + blockIdx.x * 256 + c] = s;
+}
+
+// Embedding backward as "sort, then one owner per table row".  sort_rows_kernel orders the token rows by table row:
+// it sorts the unique keys table_row * M + token_row (bitonic, one CTA, in shared memory), so the rows of one table
+// row end up adjacent and in token order.  sorted_piece_sum_kernel cuts the sorted rows into tiles of SORT_TILE; a
+// piece (the rows of one table row inside one tile) is summed in order and stored at ws[first row of the piece].
+// sorted_run_finish_kernel: the first sorted row of each table row adds the pieces of its run in order (one per tile
+// the run touches) and does the single read-modify-write of that table row.  Long runs ([PAD] in a padded batch, the
+// two token-type rows) thus cost one tile sum plus one add per tile rather than a serial walk.
+constexpr int SORT_THREADS = 1024;
+constexpr int SORT_CAP = 32768;       // token rows per sort: 128 KB of shared memory
+constexpr int SORT_TILE = 64;
+
+__global__ void __launch_bounds__(SORT_THREADS)
+sort_rows_kernel(const int* __restrict__ key, int key_mod, int row0, int M, unsigned* __restrict__ out) {
+  extern __shared__ unsigned sk[];
+  int N = 1;
+  while (N < M) N <<= 1;
+  for (int i = threadIdx.x; i < N; i += SORT_THREADS)
+    sk[i] = i < M ? (unsigned)(key != nullptr ? key[i] : (row0 + i) % key_mod) * (unsigned)M + (unsigned)i : 0xFFFFFFFFu;
+  __syncthreads();
+  for (int k = 2; k <= N; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < N; i += SORT_THREADS) {
+        const int q = i ^ j;
+        if (q > i) {
+          const unsigned a = sk[i], b = sk[q];
+          if ((a > b) == ((i & k) == 0)) { sk[i] = b; sk[q] = a; }
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (int i = threadIdx.x; i < M; i += SORT_THREADS) out[i] = sk[i];
+}
+
+// block: SORT_TILE sorted rows x 1024 columns (128 threads x 8)
+__global__ void __launch_bounds__(128)
+sorted_piece_sum_kernel(const __nv_bfloat16* __restrict__ de, const unsigned* __restrict__ sorted, int M, int H,
+                        float* __restrict__ ws) {
+  __shared__ unsigned sk[SORT_TILE];
+  const int p0 = blockIdx.x * SORT_TILE, n = min(M - p0, SORT_TILE);
+  if (threadIdx.x < n) sk[threadIdx.x] = sorted[p0 + threadIdx.x];
+  __syncthreads();
+  const int col = (blockIdx.y * 128 + threadIdx.x) * 8;
+  if (col >= H) return;
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  int head = 0;
+  auto flush = [&](int at) {
+    float4* d = reinterpret_cast<float4*>(ws + (size_t)(p0 + at) * H + col);
+    d[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    d[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+#pragma unroll
+    for (int t = 0; t < 8; ++t) acc[t] = 0.f;
+  };
+  for (int g = 0; g < n; g += 8) {           // eight row loads in flight, then the adds in sorted order
+    uint4 u[8];
+#pragma unroll
+    for (int t = 0; t < 8; ++t)
+      if (g + t < n) u[t] = ld_stream16(de + (size_t)(sk[g + t] % (unsigned)M) * H + col);
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+      const int i = g + t;
+      if (i >= n) break;
+      if (i > 0 && sk[i] / (unsigned)M != sk[i - 1] / (unsigned)M) { flush(head); head = i; }
+      float f[8];
+      unpack8(u[t], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] += f[j];
+    }
+  }
+  flush(head);
+}
+
+// grid (M, ceil(H / 1024)): block p is a no-op unless sorted row p is the first of its table row
+__global__ void __launch_bounds__(128)
+sorted_run_finish_kernel(const unsigned* __restrict__ sorted, const float* __restrict__ ws, int M, int H,
+                         float* __restrict__ table) {
+  const int p = blockIdx.x;
+  const unsigned key = sorted[p] / (unsigned)M;
+  if (p > 0 && sorted[p - 1] / (unsigned)M == key) return;
+  const int col = (blockIdx.y * 128 + threadIdx.x) * 8;
+  if (col >= H) return;
+  const float4* w0 = reinterpret_cast<const float4*>(ws + (size_t)p * H + col);
+  float4 a = w0[0], b = w0[1];
+  for (int q = (p / SORT_TILE + 1) * SORT_TILE; q < M && sorted[q] / (unsigned)M == key; q += SORT_TILE) {
+    const float4* w = reinterpret_cast<const float4*>(ws + (size_t)q * H + col);
+    const float4 c = w[0], d = w[1];
+    a.x += c.x; a.y += c.y; a.z += c.z; a.w += c.w;
+    b.x += d.x; b.y += d.y; b.z += d.z; b.w += d.w;
+  }
+  float4* t = reinterpret_cast<float4*>(table + (size_t)key * H + col);
+  float4 x = t[0], y = t[1];
+  x.x += a.x; x.y += a.y; x.z += a.z; x.w += a.w;
+  y.x += b.x; y.y += b.y; y.z += b.z; y.w += b.w;
+  t[0] = x; t[1] = y;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -872,7 +1048,7 @@ int ln_bwd_workspace_floats(int M, int H) { return ln_bwd_grid(M, H) * 3 * H; }
 void layer_norm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const float* gamma, void* dx,
                     void* dxd, float* dgamma, float* dbeta, float* dbias, float* workspace, int M, int H,
                     Seed seed, unsigned int drop_stream, unsigned int in_stream, float p_drop, Fp8Out f8,
-                    cudaStream_t st, const uint8_t* keep_mask) {
+                    cudaStream_t st, const uint8_t* keep_mask, bool deterministic) {
   unsigned int th; float sc;
   drop_params(p_drop, th, sc);
   decltype(&ln_bwd3_kernel<1, 8, false, false>) k;
@@ -894,7 +1070,9 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
   launch_pdl(k, dim3(grid), dim3(wpr * ln_bwd_groups(H) * 32), 0, st, (const __nv_bfloat16*)dy,
              (const __nv_bfloat16*)x, mean, rstd, gamma, (__nv_bfloat16*)dx, (__nv_bfloat16*)dxd, workspace, M, seed,
              drop_stream, th, sc, keep_mask, H, in_stream, f8);
-  launch_pdl(colsum_finalize_kernel, dim3((H + 31) / 32, 3, 8), dim3(256), 0, st, (const float*)workspace, grid, H,
+  // deterministic: one slice, so every column is finished by a plain += in a fixed order
+  launch_pdl(colsum_finalize_kernel, dim3((H + 31) / 32, 3, deterministic ? 1 : 8), dim3(256), 0, st,
+             (const float*)workspace, grid, H,
              dgamma, dbeta, dxd ? dbias : (float*)nullptr);
 }
 
@@ -939,8 +1117,18 @@ void gelu_fwd(const void* x, void* y, long long n, Fp8Out f8, cudaStream_t st) {
   if (g > num_sms() * 32) g = num_sms() * 32;
   if (g > 0) gelu_fwd_kernel<<<(unsigned)g, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, n8, f8);
 }
-void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int N, Fp8Out f8, cudaStream_t st) {
-  dim3 grid((N + 255) / 256, M >= 4096 ? 74 : (M >= 512 ? 16 : 1));
+static inline int dgelu_rows(int M) { return M >= 4096 ? 74 : (M >= 512 ? 16 : 1); }
+int dgelu_det_workspace_floats(int M, int N) { return dgelu_rows(M) * N; }
+
+void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int N, Fp8Out f8, cudaStream_t st,
+               float* dbias_ws) {
+  dim3 grid((N + 255) / 256, dgelu_rows(M));
+  if (dbias != nullptr && dbias_ws != nullptr) {
+    dgelu_bwd_part_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, (__nv_bfloat16*)dx,
+                                                dbias_ws, M, N, f8);
+    ordered_sum(dbias_ws, grid.y, N, nullptr, 1, dbias, st);
+    return;
+  }
   dgelu_bwd_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, (__nv_bfloat16*)dx, dbias, M, N, f8);
 }
 
@@ -976,6 +1164,54 @@ void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float
   if (grid > 0)
     embed_bwd_scatter_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)de, ids, seg, gword, gpos, gtype, M, S, H,
                                                    pos_ids);
+}
+
+void ordered_sum(const float* part, int rows, int W, const int* row_seg, int nseg, float* out, cudaStream_t st) {
+  int cw = 1;
+  while (cw < W && cw < 32) cw <<= 1;
+  if (W > 0 && nseg > 0)
+    ordered_sum_kernel<<<dim3((W + cw - 1) / cw, nseg), ORD_THREADS, 0, st>>>(part, rows, W, cw, row_seg, out);
+}
+
+static inline int colsum_rows(int M) { return M >= 4096 ? 64 : (M >= 512 ? 16 : 1); }
+int colsum_det_workspace_floats(int M, int N) { return colsum_rows(M) * N; }
+
+void colsum_bf16_det(const void* x, int M, int N, int ld, float* out, float* ws, cudaStream_t st) {
+  const int rows = colsum_rows(M);
+  colsum_bf16_part_kernel<<<dim3((N + 255) / 256, rows), 256, 0, st>>>((const __nv_bfloat16*)x, M, N, ld, ws);
+  ordered_sum(ws, rows, N, nullptr, 1, out, st);
+}
+
+int embedding_det_chunk_rows() { return SORT_CAP; }
+
+// table[key(i)] += de[i] for the M token rows i of a chunk that starts at row row0; key(i) = key[i], or
+// (row0 + i) % key_mod without key (de and key point at the chunk)
+static void sorted_scatter(const void* de, const int* key, int key_mod, int row0, int M, int H, float* table,
+                           unsigned* sort_ws, float* sum_ws, cudaStream_t st) {
+  static bool configured = false;
+  if (!configured) {
+    B200_CUDA_CHECK(cudaFuncSetAttribute(sort_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         SORT_CAP * (int)sizeof(unsigned)));
+    configured = true;
+  }
+  int n = 1;
+  while (n < M) n <<= 1;
+  sort_rows_kernel<<<1, SORT_THREADS, n * sizeof(unsigned), st>>>(key, key_mod, row0, M, sort_ws);
+  const dim3 g2((M + SORT_TILE - 1) / SORT_TILE, (H + 1023) / 1024);
+  sorted_piece_sum_kernel<<<g2, 128, 0, st>>>((const __nv_bfloat16*)de, sort_ws, M, H, sum_ws);
+  sorted_run_finish_kernel<<<dim3(M, (H + 1023) / 1024), 128, 0, st>>>(sort_ws, sum_ws, M, H, table);
+}
+
+void embedding_bwd_det(const void* de, const int* ids, const int* seg, float* gword, float* gpos, float* gtype,
+                       int M, int S, int H, const int* pos_ids, unsigned* sort_ws, float* sum_ws, cudaStream_t st) {
+  // chunks of at most SORT_CAP rows, each added to the tables in row order; a null seg keys every row to type row 0
+  for (int r0 = 0; r0 < M; r0 += SORT_CAP) {
+    const int m = M - r0 < SORT_CAP ? M - r0 : SORT_CAP;
+    const void* d = (const __nv_bfloat16*)de + (size_t)r0 * H;
+    sorted_scatter(d, ids + r0, 0, r0, m, H, gword, sort_ws, sum_ws, st);
+    sorted_scatter(d, pos_ids ? pos_ids + r0 : nullptr, S, r0, m, H, gpos, sort_ws, sum_ws, st);
+    if (gtype != nullptr) sorted_scatter(d, seg ? seg + r0 : nullptr, 1, r0, m, H, gtype, sort_ws, sum_ws, st);
+  }
 }
 
 void mlm_compact(const int* labels, int B, int S, int max_pred, int* idx, int* tgt, int* count, cudaStream_t st,

@@ -69,6 +69,25 @@ mt_l2norm_kernel(const long long* __restrict__ ptrs, const int* __restrict__ chu
   }
 }
 
+// deterministic mode: chunk c stores its sum of squares to chunk_sq[c]; ordered_sum finishes per tensor and in total
+template <typename T>
+__global__ void __launch_bounds__(OPT_THREADS)
+mt_l2norm_part_kernel(const long long* __restrict__ ptrs, const int* __restrict__ chunk_tensor,
+                      const long long* __restrict__ chunk_start, const int* __restrict__ chunk_len,
+                      float* __restrict__ chunk_sq) {
+  __shared__ float sm[32];
+  const int c = blockIdx.x;
+  const T* p = reinterpret_cast<const T*>(ptrs[chunk_tensor[c]]) + chunk_start[c];
+  const int n = chunk_len[c];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const float v = to_f<T>(p[i]);
+    s += v * v;
+  }
+  s = block_sum(s, sm);
+  if (threadIdx.x == 0) chunk_sq[c] = s;
+}
+
 template <typename TI, typename TO>
 __global__ void __launch_bounds__(OPT_THREADS)
 mt_scale_kernel(const long long* __restrict__ in_ptrs, const long long* __restrict__ out_ptrs,
@@ -94,9 +113,10 @@ mt_scale_kernel(const long long* __restrict__ in_ptrs, const long long* __restri
 // arena kernels
 // ------------------------------------------------------------------------------------------------
 // stats[0] = sum (g*inv_scale)^2, found_inf set to 1 on inf/nan.  Grid-stride over the whole arena.
-__global__ void __launch_bounds__(OPT_THREADS)
-flat_sumsq_kernel(const float* __restrict__ g, long long n, const float* __restrict__ inv_scale,
-                  float* __restrict__ stats, float* __restrict__ found_inf) {
+// PART (deterministic mode): block b stores its sum to stats[b] for ordered_sum instead of adding it to stats[0]
+template <bool PART>
+__device__ __forceinline__ void flat_sumsq_body(const float* __restrict__ g, long long n, const float* __restrict__ inv_scale,
+                                                float* __restrict__ stats, float* __restrict__ found_inf) {
   __shared__ float sm[32];
   const float is = inv_scale ? *inv_scale : 1.f;
   float s = 0.f;
@@ -111,8 +131,21 @@ flat_sumsq_kernel(const float* __restrict__ g, long long n, const float* __restr
     s += q;
   }
   s = block_sum(s, sm);
-  if (threadIdx.x == 0) atomicAdd(stats, s);
+  if constexpr (PART) { if (threadIdx.x == 0) stats[blockIdx.x] = s; }
+  else if (threadIdx.x == 0) atomicAdd(stats, s);
   if (bad && found_inf) *found_inf = 1.f;
+}
+
+__global__ void __launch_bounds__(OPT_THREADS)
+flat_sumsq_kernel(const float* __restrict__ g, long long n, const float* __restrict__ inv_scale,
+                  float* __restrict__ stats, float* __restrict__ found_inf) {
+  flat_sumsq_body<false>(g, n, inv_scale, stats, found_inf);
+}
+
+__global__ void __launch_bounds__(OPT_THREADS)
+flat_sumsq_part_kernel(const float* __restrict__ g, long long n, const float* __restrict__ inv_scale,
+                       float* __restrict__ block_sq, float* __restrict__ found_inf) {
+  flat_sumsq_body<true>(g, n, inv_scale, block_sq, found_inf);
 }
 
 // grads *= inv_scale in place + inf flag (GradScaler.unscale_ for the K-FAC path)
@@ -139,15 +172,21 @@ struct LambHyper {
 };
 
 // stage 1 over chunks of the arena; u overwrites g; norms[t] = {sum p^2, sum u^2}
-__global__ void __launch_bounds__(OPT_THREADS)
-lamb_stage1_kernel(float* __restrict__ g, const float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
-                   const int* __restrict__ chunk_tensor, const long long* __restrict__ chunk_start,
-                   const int* __restrict__ chunk_len, const int* __restrict__ decay_flag,
-                   const float* __restrict__ stats, const float* __restrict__ inv_scale,
-                   const float* __restrict__ found_inf, float* __restrict__ norms, LambHyper h) {
+// PART (deterministic mode): chunk c stores {sum p^2, sum u^2} to norms[2 c], norms[2 c + 1] for ordered_sum
+template <bool PART>
+__device__ __forceinline__ void lamb_stage1_body(float* __restrict__ g, const float* __restrict__ p, float* __restrict__ m,
+                                                 float* __restrict__ v, const int* __restrict__ chunk_tensor,
+                                                 const long long* __restrict__ chunk_start,
+                                                 const int* __restrict__ chunk_len, const int* __restrict__ decay_flag,
+                                                 const float* __restrict__ stats, const float* __restrict__ inv_scale,
+                                                 const float* __restrict__ found_inf, float* __restrict__ norms,
+                                                 const LambHyper& h) {
   __shared__ float sm[32];
-  if (found_inf && *found_inf != 0.f) return;
   const int c = blockIdx.x;
+  if (found_inf && *found_inf != 0.f) {
+    if constexpr (PART) if (threadIdx.x == 0) norms[2 * c] = norms[2 * c + 1] = 0.f;
+    return;
+  }
   const int t = chunk_tensor[c];
   const long long off = chunk_start[c];
   const int n = chunk_len[c];
@@ -197,10 +236,32 @@ lamb_stage1_kernel(float* __restrict__ g, const float* __restrict__ p, float* __
   }
   sp = block_sum(sp, sm);
   su = block_sum(su, sm);
-  if (threadIdx.x == 0) {
+  if constexpr (PART) {
+    if (threadIdx.x == 0) { norms[2 * c] = sp; norms[2 * c + 1] = su; }
+  } else if (threadIdx.x == 0) {
     atomicAdd(norms + 2 * t, sp);
     atomicAdd(norms + 2 * t + 1, su);
   }
+}
+
+__global__ void __launch_bounds__(OPT_THREADS)
+lamb_stage1_kernel(float* __restrict__ g, const float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
+                   const int* __restrict__ chunk_tensor, const long long* __restrict__ chunk_start,
+                   const int* __restrict__ chunk_len, const int* __restrict__ decay_flag,
+                   const float* __restrict__ stats, const float* __restrict__ inv_scale,
+                   const float* __restrict__ found_inf, float* __restrict__ norms, LambHyper h) {
+  lamb_stage1_body<false>(g, p, m, v, chunk_tensor, chunk_start, chunk_len, decay_flag, stats, inv_scale, found_inf,
+                          norms, h);
+}
+
+__global__ void __launch_bounds__(OPT_THREADS)
+lamb_stage1_part_kernel(float* __restrict__ g, const float* __restrict__ p, float* __restrict__ m, float* __restrict__ v,
+                        const int* __restrict__ chunk_tensor, const long long* __restrict__ chunk_start,
+                        const int* __restrict__ chunk_len, const int* __restrict__ decay_flag,
+                        const float* __restrict__ stats, const float* __restrict__ inv_scale,
+                        const float* __restrict__ found_inf, float* __restrict__ chunk_norms, LambHyper h) {
+  lamb_stage1_body<true>(g, p, m, v, chunk_tensor, chunk_start, chunk_len, decay_flag, stats, inv_scale, found_inf,
+                         chunk_norms, h);
 }
 
 // stage 2: apply, refresh shadow, zero the gradient arena slot
@@ -270,8 +331,17 @@ adam_kernel(float* __restrict__ g, float* __restrict__ p, float* __restrict__ m,
 // launchers
 // ------------------------------------------------------------------------------------------------
 void mt_l2norm(int dtype, const long long* ptrs, const int* chunk_tensor, const long long* chunk_start,
-               const int* chunk_len, int nchunks, float* per_tensor_sq, float* total_sq, cudaStream_t st) {
+               const int* chunk_len, int nchunks, float* per_tensor_sq, float* total_sq, cudaStream_t st,
+               float* chunk_ws, int ntensors) {
   if (nchunks <= 0) return;
+  if (chunk_ws != nullptr) {
+    if (dtype == 0) mt_l2norm_part_kernel<float><<<nchunks, OPT_THREADS, 0, st>>>(ptrs, chunk_tensor, chunk_start, chunk_len, chunk_ws);
+    else if (dtype == 1) mt_l2norm_part_kernel<__nv_bfloat16><<<nchunks, OPT_THREADS, 0, st>>>(ptrs, chunk_tensor, chunk_start, chunk_len, chunk_ws);
+    else mt_l2norm_part_kernel<__half><<<nchunks, OPT_THREADS, 0, st>>>(ptrs, chunk_tensor, chunk_start, chunk_len, chunk_ws);
+    if (per_tensor_sq) ordered_sum(chunk_ws, nchunks, 1, chunk_tensor, ntensors, per_tensor_sq, st);
+    ordered_sum(chunk_ws, nchunks, 1, nullptr, 1, total_sq, st);
+    return;
+  }
   if (dtype == 0) mt_l2norm_kernel<float><<<nchunks, OPT_THREADS, 0, st>>>(ptrs, chunk_tensor, chunk_start, chunk_len, per_tensor_sq, total_sq);
   else if (dtype == 1) mt_l2norm_kernel<__nv_bfloat16><<<nchunks, OPT_THREADS, 0, st>>>(ptrs, chunk_tensor, chunk_start, chunk_len, per_tensor_sq, total_sq);
   else mt_l2norm_kernel<__half><<<nchunks, OPT_THREADS, 0, st>>>(ptrs, chunk_tensor, chunk_start, chunk_len, per_tensor_sq, total_sq);
@@ -294,9 +364,18 @@ void mt_scale(int in_dtype, int out_dtype, const long long* in_ptrs, const long 
   else mt_scale_out<__half>(out_dtype, in_ptrs, out_ptrs, chunk_tensor, chunk_start, chunk_len, nchunks, scale_dev, scale_host, overflow, st);
 }
 
-void flat_sumsq(const float* g, long long n, const float* inv_scale, float* stats, float* found_inf, cudaStream_t st) {
+int flat_sumsq_det_blocks() { return 512; }
+
+void flat_sumsq(const float* g, long long n, const float* inv_scale, float* stats, float* found_inf, cudaStream_t st,
+                float* block_ws) {
   B200_CUDA_CHECK(cudaMemsetAsync(stats, 0, sizeof(float), st));
-  flat_sumsq_kernel<<<num_sms() * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, stats, found_inf);
+  if (block_ws == nullptr) {
+    flat_sumsq_kernel<<<num_sms() * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, stats, found_inf);
+    return;
+  }
+  // a fixed grid: the block partition of the sum does not depend on the device either
+  flat_sumsq_part_kernel<<<flat_sumsq_det_blocks(), OPT_THREADS, 0, st>>>(g, n, inv_scale, block_ws, found_inf);
+  ordered_sum(block_ws, flat_sumsq_det_blocks(), 1, nullptr, 1, stats, st);
 }
 void flat_unscale(float* g, long long n, const float* inv_scale, float* found_inf, cudaStream_t st) {
   flat_unscale_kernel<<<num_sms() * 4, OPT_THREADS, 0, st>>>(g, n, inv_scale, found_inf);
@@ -306,7 +385,8 @@ void arena_lamb(float* g, float* p, float* m, float* v, void* shadow, const int*
                 const long long* chunk_start, const int* chunk_len, int nchunks, const int* decay_flag,
                 int ntensors, float* stats, float* norms, const float* inv_scale, const float* found_inf,
                 float lr, float beta1, float beta2, float eps, float weight_decay, int step, int bias_correction,
-                int grad_averaging, float max_grad_norm, int adam_w_mode, int use_nvlamb, cudaStream_t st) {
+                int grad_averaging, float max_grad_norm, int adam_w_mode, int use_nvlamb, cudaStream_t st,
+                float* chunk_ws) {
   LambHyper h;
   h.lr = lr; h.beta1 = beta1; h.beta2 = beta2; h.beta3 = grad_averaging ? 1.f - beta1 : 1.f; h.eps = eps;
   h.weight_decay = weight_decay;
@@ -314,8 +394,14 @@ void arena_lamb(float* g, float* p, float* m, float* v, void* shadow, const int*
   h.bc2 = bias_correction ? 1.f - powf(beta2, (float)step) : 1.f;
   h.max_grad_norm = max_grad_norm; h.adam_w_mode = adam_w_mode; h.use_nvlamb = use_nvlamb;
   B200_CUDA_CHECK(cudaMemsetAsync(norms, 0, sizeof(float) * 2 * ntensors, st));
-  lamb_stage1_kernel<<<nchunks, OPT_THREADS, 0, st>>>(g, p, m, v, chunk_tensor, chunk_start, chunk_len, decay_flag,
-                                                     stats, inv_scale, found_inf, norms, h);
+  if (chunk_ws == nullptr) {
+    lamb_stage1_kernel<<<nchunks, OPT_THREADS, 0, st>>>(g, p, m, v, chunk_tensor, chunk_start, chunk_len, decay_flag,
+                                                       stats, inv_scale, found_inf, norms, h);
+  } else {
+    lamb_stage1_part_kernel<<<nchunks, OPT_THREADS, 0, st>>>(g, p, m, v, chunk_tensor, chunk_start, chunk_len,
+                                                            decay_flag, stats, inv_scale, found_inf, chunk_ws, h);
+    ordered_sum(chunk_ws, nchunks, 2, chunk_tensor, ntensors, norms, st);
+  }
   lamb_stage2_kernel<<<nchunks, OPT_THREADS, 0, st>>>(g, p, (__nv_bfloat16*)shadow, chunk_tensor, chunk_start,
                                                      chunk_len, decay_flag, found_inf, norms, h);
 }

@@ -33,6 +33,7 @@ import numpy as np
 import torch
 
 from . import models as modeling
+from . import ops
 from .config import BertConfig, batch_arithmetic, overlay_json_config
 from .data import BatchedPretrainingLoader, DistributedSampler, ShardedPretrainingDataset
 from .data.tokenization import get_bpe_tokenizer, get_wordpiece_tokenizer
@@ -103,6 +104,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--unpad", default=False, action="store_true",
                    help="fused engine: compute only the unmasked tokens of each micro-batch (packed on the device into "
                         "one of 16 token buckets, one CUDA graph per bucket); fp8 operands run padded")
+    p.add_argument("--deterministic", default=False, action="store_true",
+                   help="fused engine: bitwise-reproducible training: the fused engine's fixed-order reductions (no "
+                        "floating-point atomics) and torch.use_deterministic_algorithms(True); the same program on the "
+                        "same inputs, GPU and build gives the same loss, gradients and weights")
     return p
 
 
@@ -124,6 +129,12 @@ def check_required(args) -> None:
 # ---------------------------------------------------------------------------
 
 def setup_training(args):
+    if getattr(args, "deterministic", False):
+        if args.backend == "fused":
+            # its GEMMs push weight-gradient tiles into the owner rank's arena with atomics, and its fused LAMB step
+            # reduces across ranks: neither has a fixed order, and the in-order split-K partials cannot be pushed
+            raise ValueError("--deterministic covers one GPU and cannot be combined with --backend fused")
+        ops.use_deterministic()
     use_cuda = torch.cuda.is_available() if args.device is None else args.device == "cuda"
     if use_cuda:
         torch.cuda.set_device(args.local_rank)
