@@ -293,6 +293,90 @@ class ShardedPretrainingDataset(torch.utils.data.Dataset):
 
 
 # ---------------------------------------------------------------------------
+# held-out evaluation set
+# ---------------------------------------------------------------------------
+
+
+class HeldOutSet:
+    """A fixed evaluation set: the first ``num_examples`` samples of ``files`` (sorted, as for training), masked once
+    at construction and held as five int32 host tensors ``[input_ids, segment_ids, input_mask, masked_lm_labels,
+    next_sentence_labels]`` (pinned with ``pin_memory``).
+
+    Shards with dynamic masking: sample ``i`` is masked by a generator seeded from ``(seed, i)``, so the set does not
+    depend on the world size, the batch size or how often it is evaluated.  Pre-masked (legacy schema) shards keep
+    their stored masks.  Masking follows the training settings, and the training check of pre-masked shards against
+    ``max_pred_per_seq`` applies."""
+
+    def __init__(self, files, num_examples: int, mask_token_index: Optional[int], max_pred_per_seq: int,
+                 masked_lm_prob: float, vocab_size: int, seed: int = 0, original_token_prob: float = 0.1,
+                 random_token_prob: float = 0.1, pin_memory: bool = False):
+        if num_examples < 1:
+            raise ValueError("num_examples must be at least 1")
+        ds = ShardedPretrainingDataset(files, mask_token_index, max_pred_per_seq, masked_lm_prob, vocab_size,
+                                       original_token_prob=original_token_prob, random_token_prob=random_token_prob)
+        n = min(int(num_examples), len(ds))
+        self.seed = int(seed)
+        kw = dict(mask_token_index=mask_token_index, max_pred_per_seq=int(max_pred_per_seq),
+                  masked_lm_prob=float(masked_lm_prob), vocab_size=int(vocab_size),
+                  original_token_prob=original_token_prob, random_token_prob=random_token_prob)
+        cols: List[List[np.ndarray]] = [[] for _ in range(5)]
+        for fi, (f_lo, f_hi) in enumerate(ds.file_idxs):
+            if f_lo >= n:
+                break
+            hi = min(f_hi, n) - f_lo
+            d = ds.shard(fi)
+            if "special_token_positions" in d:
+                ids = np.asarray(d["input_ids"][:hi])
+                sp = np.asarray(d["special_token_positions"][:hi])
+                seg, imask = segment_ids_and_input_mask(ids, sp)
+                masked, labels = np.empty_like(ids), np.empty_like(ids)
+                for r in range(hi):
+                    rng = np.random.default_rng([self.seed, f_lo + r])
+                    masked[r:r + 1], labels[r:r + 1] = mask_batch(ids[r:r + 1], sp[r:r + 1], rng=rng, **kw)
+                out = [masked, seg, imask, labels, np.asarray(d["next_sentence_labels"][:hi])]
+            else:
+                out = ds.build_batch(fi, 0, hi)
+            for c in range(5):
+                cols[c].append(np.asarray(out[c]))
+        self.tensors = []
+        for c in cols:
+            t = torch.from_numpy(np.ascontiguousarray(np.concatenate(c, axis=0))).to(torch.int32)
+            self.tensors.append(t.pin_memory() if pin_memory else t)
+        self.pin = bool(pin_memory)
+
+    def __len__(self) -> int:
+        return self.tensors[0].size(0)
+
+    def rank_range(self, rank: int = 0, world: int = 1) -> Tuple[int, int]:
+        """The contiguous slice ``[lo, hi)`` of the samples that rank ``rank`` of ``world`` evaluates."""
+        n = len(self)
+        return rank * n // world, (rank + 1) * n // world
+
+    def batches(self, batch_size: int, rank: int = 0, world: int = 1) -> Iterator[List[torch.Tensor]]:
+        """This rank's samples in batches of ``batch_size``.  The last batch is filled up with inert rows (every label
+        -1, only the first token unmasked), so that one shape serves every batch and, unpadded, a filler row costs one
+        token."""
+        lo, hi = self.rank_range(rank, world)
+        for i in range(lo, hi, batch_size):
+            j = min(i + batch_size, hi)
+            batch = [t[i:j] for t in self.tensors]
+            if j - i < batch_size:
+                batch = [torch.cat([t, self.filler(t, batch_size - (j - i), c)]) for c, t in enumerate(batch)]
+                batch = [t.pin_memory() if self.pin else t for t in batch]
+            yield batch
+
+    @staticmethod
+    def filler(like: torch.Tensor, rows: int, column: int) -> torch.Tensor:
+        """``rows`` inert rows of input column ``column``: labels -1, the attention mask 1 at the first token only."""
+        t = torch.zeros((rows,) + tuple(like.shape[1:]), dtype=like.dtype)
+        if column == 2:
+            t[:, 0] = 1
+        elif column in (3, 4):
+            t.fill_(-1)
+        return t
+
+
+# ---------------------------------------------------------------------------
 # sampler
 # ---------------------------------------------------------------------------
 

@@ -735,6 +735,7 @@ class FusedPretrainer:
         self._cls_idx = None                  # row indices of the [CLS] tokens (NSP head)
         self._cap_stream = None               # high-priority capture stream (wgrad side-stream mode)
         self._cls_S = 0
+        self._eval_cls: Dict[tuple, torch.Tensor] = {}   # [CLS] row indices of the evaluation batch shapes
 
     def _max_pred(self, labels: torch.Tensor) -> int:
         # capacity of masked positions per sequence; fixed per run so shapes stay static
@@ -751,11 +752,11 @@ class FusedPretrainer:
             return False                      # tapped micro-steps keep Python-side state; the library attention path owns its RNG
         return self.arena.device.type == "cuda"
 
-    def _bucket(self, input_mask, tokens: Optional[int]):
+    def _bucket(self, input_mask, tokens: Optional[int], kfac: bool = True):
         """(T_cap, D) of this micro-step when it runs unpadded (``BertModel.unpad``), else None.  fp8 operands and the
         library attention have no unpadded path (warned once), and K-FAC micro-steps that feed the factors run padded
-        so that their statistics are the padded ones.  Without ``tokens`` the count is read back from the device (one
-        host sync)."""
+        so that their statistics are the padded ones (``kfac=False``: an evaluation, which feeds nothing).  Without
+        ``tokens`` the count is read back from the device (one host sync)."""
         if not getattr(self.model.bert, "unpad", False):
             return None
         eng = self.engine
@@ -766,7 +767,7 @@ class FusedPretrainer:
                 self._unpad_warned = True
             return None
         kf = getattr(self.model.bert, "_kfac", None)
-        if kf is not None and getattr(kf, "capture", True):
+        if kfac and kf is not None and getattr(kf, "capture", True):
             return None
         B, S = input_mask.shape
         return token_bucket(packed_tokens(input_mask) if tokens is None else int(tokens), B, S)
@@ -922,3 +923,110 @@ class FusedPretrainer:
 
         eng.backward(sv, d_seq)
         return loss.squeeze(0) if loss.dim() else loss
+
+    # -- evaluation ------------------------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def evaluate(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels, acc: torch.Tensor,
+                 tokens: Optional[int] = None) -> torch.Tensor:
+        """Adds the metric sums of one batch into ``acc`` (fp64 [6] on the device): ``[mlm_loss_sum, mlm_correct,
+        mlm_count, nsp_loss_sum, nsp_correct, nsp_count]`` (the NSP half stays zero without an NSP head or labels).
+        Forward only, without dropout, and every sum in a fixed order (no atomics): the same batch gives the same bits in
+        the default and the deterministic mode, padded or unpadded, eager or replayed.
+
+        The training state comes out as it went in: no activation is saved, no gradient is written, the dropout seed
+        counters (``_seed_step``, the engine's call count) and ``model.training`` do not move, and the fp8 scaling table
+        is restored after the batch (the weight copies are refreshed first, as the next micro-step would).  Unpadded
+        (``BertModel.unpad``) the batch is packed into the token bucket of ``tokens`` as in training.  CUDA graphs: the
+        training policy (``graph_warmup`` eager calls per signature, then one capture), with keys of their own in the
+        training graphs' memory pool."""
+        if acc.dtype != torch.float64 or acc.numel() != 6:
+            raise ValueError("evaluate: acc must be an fp64 tensor of 6 elements")
+        eng = self.engine
+        bucket = self._bucket(input_mask, tokens, kfac=False)
+        args = (input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels)
+        table = None
+        if eng.fp8:
+            eng.prepare_step()
+            table = eng.meta.table.clone()
+        try:
+            part = self._eval_replay(args, bucket)
+            acc += part
+        finally:
+            if table is not None:
+                eng.meta.table.copy_(table)
+        return acc
+
+    def _eval_replay(self, args, bucket) -> torch.Tensor:
+        """The evaluation program of ``args``, eager or as a replayed CUDA graph; returns its fp64 [6] sums."""
+        eng = self.engine
+        if not (self.use_graphs and not _use_sdpa() and self.arena.device.type == "cuda"):
+            return self._eval_program(*args, bucket=bucket)
+        input_ids, segment_ids, _, _, next_sentence_labels = args
+        key = ("eval", tuple(input_ids.shape), next_sentence_labels is not None, segment_ids is not None,
+               tuple(str(t.dtype) for t in args if t is not None), eng.fp8, K.deterministic(), bucket)
+        ent = self._graphs.setdefault(key, {"calls": 0})
+        ent["calls"] += 1
+        if "graph" not in ent:
+            if ent["calls"] <= self.graph_warmup or (eng.fp8 and not eng._fp8_calibrated):
+                return self._eval_program(*args, bucket=bucket)
+            self._max_pred(args[3].to(torch.int32))
+            static = [None if t is None else t.clone() for t in args]
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            n0 = K.KERNEL_LAUNCHES
+            pool = next((e["graph"].pool() for e in self._graphs.values() if "graph" in e), None)
+            try:
+                # no seed-step increment in here: the program has no dropout, and training's counter must not move
+                with torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local"):
+                    part = self._eval_program(*static, bucket=bucket)
+            except Exception as e:
+                warnings.warn(f"CUDA-graph capture of the evaluation failed ({type(e).__name__}: {e}); "
+                              "continuing with the eager kernel program")
+                K.KERNEL_LAUNCHES = n0
+                self.use_graphs = False
+                torch.cuda.synchronize()
+                return self._eval_program(*args, bucket=bucket)
+            ent.update(graph=graph, static=static, part=part, launches=K.KERNEL_LAUNCHES - n0)
+            K.KERNEL_LAUNCHES = n0
+        for dst, src in zip(ent["static"], args):
+            if dst is not None:
+                dst.copy_(src, non_blocking=True)
+        ent["graph"].replay()
+        K._count(ent["launches"])
+        return ent["part"]
+
+    @torch.no_grad()
+    def _eval_program(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
+                      bucket=None) -> torch.Tensor:
+        """Encoder forward without dropout, the MLM head on the masked rows and the NSP head on the [CLS] rows, then the
+        metric kernels.  Returns fp64 [6]: the MLM sums {loss, correct, count}, then the NSP sums."""
+        eng, A = self.engine, self.arena
+        B, S = input_ids.shape
+        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
+        # an explicit seed: the engine's call counter, which numbers the training dropout seeds, stays where it is
+        seq, _ = eng.forward(input_ids, segment_ids, input_mask, training=False, seed=0, dropout=False, pack=pk)
+        labels = masked_lm_labels.to(torch.int32).contiguous()
+        idx, tgt, _ = K.mlm_compact(labels, self._max_pred(labels), row_map=pk.row_map if pk is not None else None)
+        part = torch.zeros(6, dtype=torch.float64, device=seq.device)
+
+        rows = K.gather_rows(seq, idx)
+        t_pre = K.gemm(rows, A.shadow("cls.predictions.transform.dense_act.weight"), epi=K.EPI_BIAS,
+                       bias=A.shadow("cls.predictions.transform.dense_act.bias"))
+        t_ln, _, _ = K.layer_norm_fwd(K.gelu_fwd(t_pre), A.view("cls.predictions.transform.LayerNorm.weight"),
+                                      A.view("cls.predictions.transform.LayerNorm.bias"), save_stats=False)
+        logits = K.gemm(t_ln, eng.w("embeddings.word_embeddings.weight"), epi=K.EPI_BIAS, bias=A.shadow("cls.predictions.bias"))
+        K.mlm_eval(logits, tgt, part[0:3])
+
+        if self.has_nsp and next_sentence_labels is not None:
+            if pk is not None:
+                cls_idx = pk.cls_rows
+            else:
+                # a cache of its own: a captured training graph keeps reading the training batch's index tensor
+                cls_idx = self._eval_cls.get((B, S))
+                if cls_idx is None:
+                    cls_idx = self._eval_cls[(B, S)] = torch.arange(B, device=seq.device, dtype=torch.int32) * S
+            pooled = K.gemm(K.gather_rows(seq, cls_idx), A.shadow(eng.prefix + "pooler.dense_act.weight"),
+                            epi=K.EPI_BIAS_TANH, bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
+            K.nsp_eval(pooled, A.shadow("cls.seq_relationship.weight"), self.model.cls.seq_relationship.bias,
+                       next_sentence_labels.long().view(-1).contiguous(), part[3:6])
+        return part

@@ -572,6 +572,17 @@ class BertModel(BertPreTrainedModel):
         return layers, pooled
 
 
+def _metric_sums(scores: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+    """fp64 [3] {cross-entropy sum, correct count, count} of the rows of ``scores`` whose label is not -1
+    (``torch.argmax``: the lowest index wins a tie)."""
+    labels = labels.long().to(scores.device)
+    keep = labels >= 0
+    s, t = scores[keep].float(), labels[keep]
+    loss = F.cross_entropy(s, t, reduction="none").double().sum()
+    correct = (s.argmax(dim=-1) == t).sum().double()
+    return torch.stack([loss, correct, torch.tensor(float(t.numel()), dtype=torch.float64, device=s.device)])
+
+
 class BertForPreTraining(BertPreTrainedModel):
     """MLM + (optional) NSP heads; returns raw scores, the loss lives in the
     criterion (src/modeling.py:886-947)."""
@@ -602,6 +613,28 @@ class BertForPreTraining(BertPreTrainedModel):
             from .fused import FusedPretrainer
             self._pretrainer = FusedPretrainer(self)
         return self._pretrainer
+
+    @torch.no_grad()
+    def evaluate(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels, acc: torch.Tensor,
+                 tokens: Optional[int] = None) -> torch.Tensor:
+        """Adds the held-out metric sums of one batch into ``acc`` (fp64 [6]): ``[mlm_loss_sum, mlm_correct, mlm_count,
+        nsp_loss_sum, nsp_correct, nsp_count]`` over the rows whose label is not -1.  Through the fused engine
+        (:meth:`~.fused.FusedPretrainer.evaluate`) where it runs, else from the plain PyTorch forward with dropout off
+        (autocast is the caller's), with the same rule for ties: the lowest index wins an argmax."""
+        eng = self.pretrain_engine()
+        if eng is not None:
+            return eng.evaluate(input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels, acc,
+                                tokens=tokens)
+        was = self.training
+        self.eval()
+        try:
+            scores, nsp = self(input_ids.long(), None if segment_ids is None else segment_ids.long(), input_mask.long())
+        finally:
+            self.train(was)
+        acc[0:3] += _metric_sums(scores.reshape(-1, scores.size(-1)), masked_lm_labels.reshape(-1))
+        if nsp is not None and next_sentence_labels is not None:
+            acc[3:6] += _metric_sums(nsp.reshape(-1, 2), next_sentence_labels.reshape(-1))
+        return acc
 
 
 class BertForMaskedLM(BertPreTrainedModel):

@@ -387,6 +387,43 @@ def softmax_ce_(logits: torch.Tensor, targets: torch.Tensor, count: torch.Tensor
     _count(2 if det else 1)
 
 
+def _eval_sums(acc: Optional[torch.Tensor], sums: torch.Tensor) -> None:
+    if acc is not None:
+        if acc.dtype != torch.float64 or acc.numel() != 3:
+            raise ValueError("the metric accumulator must be an fp64 tensor of 3 elements")
+        acc += sums
+
+
+def mlm_eval(logits: torch.Tensor, targets: torch.Tensor, acc: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Masked-LM metrics of bf16 logits [R, V] (only read) against int32 ``targets`` [R] (< 0: ignored).  Returns the
+    rows fp32 [R, 3] = {loss, correct, valid}: ``logsumexp(row) - row[t]`` (the forward half of :func:`softmax_ce_`,
+    same arithmetic), ``argmax(row) == t`` with the lowest index winning a tie (``torch.argmax``'s rule), and 1; an
+    ignored row is {0, 0, 0}.  ``acc`` (fp64 [3]) += their column sums, added in a fixed order without atomics in every
+    mode: {loss sum, correct count, row count}."""
+    R = logits.size(0)
+    rows = torch.empty(R, 3, dtype=torch.float32, device=logits.device)
+    sums = torch.zeros(3, dtype=torch.float32, device=logits.device)
+    extension().mlm_eval(logits, targets, rows, sums)
+    _count(2)
+    _eval_sums(acc, sums)
+    return rows
+
+
+def nsp_eval(pooled: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, labels: torch.Tensor,
+             acc: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Next-sentence metrics of the pooled bf16 [B, H] through the classifier ``w`` bf16 [2, H] + fp32 ``bias``
+    against int64 ``labels`` [B] (< 0: ignored): rows fp32 [B, 3] = {cross-entropy, prediction == label, 1}, where the
+    prediction is class 1 only when its logit is strictly larger.  ``acc`` (fp64 [3]) += their column sums, as
+    :func:`mlm_eval`."""
+    B = pooled.size(0)
+    rows = torch.empty(B, 3, dtype=torch.float32, device=pooled.device)
+    sums = torch.zeros(3, dtype=torch.float32, device=pooled.device)
+    extension().nsp_eval(pooled, w, bias, labels, rows, sums)
+    _count(2)
+    _eval_sums(acc, sums)
+    return rows
+
+
 def _attn_shape(qkv: torch.Tensor, seqlens, cu_seqlens, S):
     """(B, S, rows, H) of the padded form (qkv [B, S, 3H], ``seqlens`` int32 [B]) or of the varlen form (qkv packed
     [T, 3H], ``cu_seqlens`` int32 [B + 1], ``S`` the padded length)."""

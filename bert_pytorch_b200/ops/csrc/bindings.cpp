@@ -609,6 +609,41 @@ void nsp_head(Tensor pooled, Tensor w, Tensor bias, Tensor labels, double grad_s
                  cur_stream(), deterministic ? f32_workspace(dw, B * (3 + 2 * H)).data_ptr<float>() : nullptr);
 }
 
+// evaluation metrics: rows fp32 [R, 3] ({loss, correct, valid} per row), sums fp32 [3] += their column sums (in order)
+inline void check_eval_out(const Tensor& rows, const Tensor& sums, int64_t R, const Tensor& like, const char* name) {
+  TORCH_CHECK(rows.is_cuda() && rows.device() == like.device() && rows.scalar_type() == at::kFloat && rows.is_contiguous() &&
+              rows.numel() == 3 * R, name, ": rows must be a contiguous fp32 CUDA tensor [R, 3]");
+  TORCH_CHECK(sums.is_cuda() && sums.device() == like.device() && sums.scalar_type() == at::kFloat && sums.is_contiguous() &&
+              sums.numel() == 3, name, ": sums must be a contiguous fp32 CUDA tensor [3]");
+}
+
+void mlm_eval(Tensor logits, Tensor targets, Tensor rows, Tensor sums) {
+  check_bf16(logits, "logits");
+  TORCH_CHECK(logits.dim() == 2 && logits.size(1) % 8 == 0 && logits.stride(0) % 8 == 0, "mlm_eval: logits [R, V], V % 8 == 0");
+  const int64_t R = logits.size(0);
+  check_i32(targets, logits, R, "mlm_eval: targets");
+  check_eval_out(rows, sums, R, logits, "mlm_eval");
+  c10::cuda::CUDAGuard guard(logits.device());
+  b200::mlm_eval(logits.data_ptr(), (int)logits.stride(0), targets.data_ptr<int>(), (int)R, (int)logits.size(1),
+                 rows.data_ptr<float>(), sums.data_ptr<float>(), cur_stream());
+}
+
+void nsp_eval(Tensor pooled, Tensor w, Tensor bias, Tensor labels, Tensor rows, Tensor sums) {
+  check_bf16(pooled, "pooled"); check_bf16(w, "w");
+  TORCH_CHECK(pooled.dim() == 2 && pooled.is_contiguous(), "nsp_eval: pooled must be a contiguous [B, H]");
+  const int64_t B = pooled.size(0), H = pooled.size(1);
+  TORCH_CHECK(w.is_contiguous() && w.dim() == 2 && w.size(0) == 2 && w.size(1) == H, "nsp_eval: w must be [2, H]");
+  TORCH_CHECK(bias.is_cuda() && bias.device() == pooled.device() && bias.scalar_type() == at::kFloat && bias.is_contiguous() &&
+              bias.numel() == 2, "nsp_eval: bias must be a contiguous fp32 CUDA tensor [2]");
+  TORCH_CHECK(labels.is_cuda() && labels.device() == pooled.device() && labels.scalar_type() == at::kLong &&
+              labels.is_contiguous() && labels.numel() == B, "nsp_eval: labels must be a contiguous int64 CUDA tensor [B]");
+  check_eval_out(rows, sums, B, pooled, "nsp_eval");
+  c10::cuda::CUDAGuard guard(pooled.device());
+  b200::nsp_eval(pooled.data_ptr(), w.data_ptr(), bias.data_ptr<float>(),
+                 reinterpret_cast<const long long*>(labels.data_ptr<int64_t>()), (int)B, (int)H, rows.data_ptr<float>(),
+                 sums.data_ptr<float>(), cur_stream());
+}
+
 void peer_allreduce(int64_t rank, int64_t world, bool use_multicast, std::vector<int64_t> buf_ptrs,
                     std::vector<int64_t> flag_ptrs, int64_t buf_mc, Tensor grid_bar, int64_t epoch, int64_t n, double scale) {
   TORCH_CHECK((int64_t)buf_ptrs.size() == world && (int64_t)flag_ptrs.size() == world && world <= 16, "peer pointer lists");
@@ -694,6 +729,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("scatter_rows", &scatter_rows);
   m.def("softmax_ce", &softmax_ce);
   m.def("nsp_head", &nsp_head);
+  m.def("mlm_eval", &mlm_eval);
+  m.def("nsp_eval", &nsp_eval);
   m.def("mt_l2norm", &mt_l2norm);
   m.def("mt_scale", &mt_scale);
   m.def("flat_sumsq", &flat_sumsq);

@@ -133,6 +133,14 @@ void nsp_head(const void* pooled_bf16, const void* w_bf16, const float* bias, co
               float grad_scale, float* loss_out, void* dz_bf16, float* dw, float* db, cudaStream_t st,
               float* rows_ws = nullptr);   // rows_ws [B * (3 + 2 H)]: deterministic mode
 
+// loss.cu: evaluation metrics, forward only.  rows [R, 3] receives {loss, correct, valid} of every row ({0, 0, 0} for an
+// ignored one); sums [3] += the column sums of rows, added by ordered_sum (no atomics, the same bits in every mode).
+// mlm_eval: bf16 logits [R, V] (V % 8 == 0, row stride ld), targets int32 (< 0: ignored).  nsp_eval: pooled bf16 [B, H],
+// classifier w bf16 [2, H], fp32 bias [2], int64 labels (< 0: ignored).
+void mlm_eval(const void* logits, int ld, const int* targets, int R, int V, float* rows, float* sums, cudaStream_t st);
+void nsp_eval(const void* pooled, const void* w, const float* bias, const long long* labels, int B, int H, float* rows,
+              float* sums, cudaStream_t st);
+
 // fp8.cu: per-tensor scaled fp8 operand preparation; meta records are {amax, scale, inv_scale, _}
 void fp8_quantize(const void* x_bf16, void* q, long long n, float* meta, bool e5m2, cudaStream_t st);
 void fp8_amax(const void* x_bf16, long long n, float* meta, cudaStream_t st);

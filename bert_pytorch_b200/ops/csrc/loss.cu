@@ -228,4 +228,156 @@ void nsp_head(const void* pooled, const void* w, const float* bias, const long l
   ordered_sum(dw_rows, B, 2 * H, nullptr, 1, dw, st);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Evaluation metrics (forward only; the inputs are only read).  Every row r writes rows[r] = {loss, correct, valid}:
+// the cross-entropy of its target, whether the argmax is the target, and 1 -- or {0, 0, 0} for an ignored row.  The
+// rows are then added by ordered_sum in a fixed order: no atomics, so the sums are the same bits in every mode.
+// ------------------------------------------------------------------------------------------------
+
+// (value, index) pair that wins an argmax: the larger value, and the lower index among equal values
+__device__ __forceinline__ void argmax_take(float& v, int& i, float ov, int oi) {
+  if (ov > v || (ov == v && oi < i)) { v = ov; i = oi; }
+}
+
+// One block per row of bf16 logits [R, V] (V % 8 == 0, row stride ld).  The loss is the forward half of
+// softmax_ce_body with the same block shape and the same arithmetic, so that both give the same per-row term.  A target
+// outside [0, V) counts as ignored.
+__global__ void __launch_bounds__(CE_THREADS)
+mlm_eval_kernel(const __nv_bfloat16* __restrict__ logits, int ld, const int* __restrict__ targets, int V,
+                float* __restrict__ rows) {
+  __shared__ float sm[32];
+  __shared__ int si[32];
+  __shared__ float s_max, s_sum;
+  __shared__ int s_arg;
+  const int r = blockIdx.x;
+  const __nv_bfloat16* row = logits + (size_t)r * ld;
+  const int tgt = targets[r];
+  if (tgt < 0 || tgt >= V) {
+    if (threadIdx.x < 3) rows[(size_t)r * 3 + threadIdx.x] = 0.f;
+    return;
+  }
+  const int nvec = V >> 3;
+  const uint4* row4 = reinterpret_cast<const uint4*>(row);
+  float m = -INFINITY, s = 0.f;
+  float bv = -INFINITY;
+  int bi = V;                        // no index yet (a row of NaN has no argmax and is never correct)
+  for (int i = threadIdx.x; i < nvec; i += CE_THREADS) {
+    const uint4 u = row4[i];
+    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+    float f[8];
+#pragma unroll
+    for (int t = 0; t < 4; ++t) {
+      const float2 p = unpack_bf16(w[t]);
+      f[2 * t] = p.x; f[2 * t + 1] = p.y;
+    }
+    float lm = f[0];
+#pragma unroll
+    for (int t = 1; t < 8; ++t) lm = fmaxf(lm, f[t]);
+    const float nm = fmaxf(m, lm);
+    float acc = 0.f;
+#pragma unroll
+    for (int t = 0; t < 8; ++t) acc += __expf(f[t] - nm);
+    s = s * __expf(m - nm) + acc;
+    m = nm;
+#pragma unroll
+    for (int t = 0; t < 8; ++t)      // a thread visits its indices in increasing order: strict > keeps the lowest
+      if (f[t] > bv) { bv = f[t]; bi = i * 8 + t; }
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // block combine of the softmax statistics: softmax_ce_body's order
+  float wm = warp_max(m);
+  if (lane == 0) sm[warp] = wm;
+  __syncthreads();
+  if (warp == 0) {
+    float v = lane < CE_THREADS / 32 ? sm[lane] : -INFINITY;
+    v = warp_max(v);
+    if (lane == 0) s_max = v;
+  }
+  __syncthreads();
+  const float gmax = s_max;
+  float part = (m == -INFINITY) ? 0.f : s * __expf(m - gmax);
+  part = warp_sum(part);
+  if (lane == 0) sm[warp] = part;
+  __syncthreads();
+  if (warp == 0) {
+    float v = lane < CE_THREADS / 32 ? sm[lane] : 0.f;
+    v = warp_sum(v);
+    if (lane == 0) s_sum = v;
+  }
+  // block combine of the argmax
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+    argmax_take(bv, bi, __shfl_xor_sync(0xffffffffu, bv, o), __shfl_xor_sync(0xffffffffu, bi, o));
+  __syncthreads();                   // sm is free again (warp 0 has read it)
+  if (lane == 0) { sm[warp] = bv; si[warp] = bi; }
+  __syncthreads();
+  if (warp == 0) {
+    float v = lane < CE_THREADS / 32 ? sm[lane] : -INFINITY;
+    int k = lane < CE_THREADS / 32 ? si[lane] : V;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+      argmax_take(v, k, __shfl_xor_sync(0xffffffffu, v, o), __shfl_xor_sync(0xffffffffu, k, o));
+    if (lane == 0) s_arg = k;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const float lt = __bfloat162float(row[tgt]);
+    rows[(size_t)r * 3 + 0] = logf(s_sum) + gmax - lt;
+    rows[(size_t)r * 3 + 1] = s_arg == tgt ? 1.f : 0.f;
+    rows[(size_t)r * 3 + 2] = 1.f;
+  }
+}
+
+void mlm_eval(const void* logits, int ld, const int* targets, int R, int V, float* rows, float* sums, cudaStream_t st) {
+  if (R <= 0) return;
+  mlm_eval_kernel<<<R, CE_THREADS, 0, st>>>((const __nv_bfloat16*)logits, ld, targets, V, rows);
+  ordered_sum(rows, R, 3, nullptr, 1, sums, st);
+}
+
+// One block per sequence: the NSP classifier and its cross-entropy with nsp_head_body's block shape and arithmetic.  The
+// prediction is class 1 only when its logit is strictly larger (a tie goes to class 0, torch.argmax's rule).
+__global__ void __launch_bounds__(128)
+nsp_eval_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w,
+                const float* __restrict__ bias, const long long* __restrict__ labels, int H, float* __restrict__ rows) {
+  __shared__ float sm[32];
+  const int b = blockIdx.x;
+  const long long y = labels[b];
+  float* out = rows + (size_t)b * 3;
+  if (y < 0 || y > 1) {
+    if (threadIdx.x < 3) out[threadIdx.x] = 0.f;
+    return;
+  }
+  const __nv_bfloat16* x = pooled + (size_t)b * H;
+  float a0 = 0.f, a1 = 0.f;
+  for (int i = threadIdx.x; i < H; i += blockDim.x) {
+    const float xv = __bfloat162float(x[i]);
+    a0 += xv * __bfloat162float(w[i]);
+    a1 += xv * __bfloat162float(w[H + i]);
+  }
+  auto block_sum = [&](float v) -> float {
+    v = warp_sum(v);
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float r = 0.f;
+    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) r += sm[k];
+    __syncthreads();
+    return r;
+  };
+  const float l0 = block_sum(a0) + bias[0], l1 = block_sum(a1) + bias[1];
+  if (threadIdx.x == 0) {
+    const float m = fmaxf(l0, l1);
+    const float lse = m + logf(expf(l0 - m) + expf(l1 - m));
+    out[0] = lse - (y == 0 ? l0 : l1);
+    out[1] = (l1 > l0 ? 1 : 0) == y ? 1.f : 0.f;
+    out[2] = 1.f;
+  }
+}
+
+void nsp_eval(const void* pooled, const void* w, const float* bias, const long long* labels, int B, int H, float* rows,
+              float* sums, cudaStream_t st) {
+  if (B <= 0) return;
+  nsp_eval_kernel<<<B, 128, 0, st>>>((const __nv_bfloat16*)pooled, (const __nv_bfloat16*)w, bias, labels, H, rows);
+  ordered_sum(rows, B, 3, nullptr, 1, sums, st);
+}
+
 }  // namespace b200

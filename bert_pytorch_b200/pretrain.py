@@ -12,7 +12,8 @@ Function names, flags, output files and checkpoint layout follow the reference
   * the loss stays on the device between micro-steps (the reference syncs the host every
     micro-step, run_pretraining.py:542); data arrives through the batched pinned loader;
   * new flags: ``--bf16`` (default compute type on CUDA), ``--fp8``, ``--backend``,
-    ``--device``, ``--no_fused``, ``--loader_depth``, ``--unpad``.
+    ``--device``, ``--no_fused``, ``--loader_depth``, ``--unpad``, and the held-out evaluation ``--eval_dir`` /
+    ``--num_eval_examples`` / ``--eval_batch_size`` / ``--eval_interval`` / ``--eval_seed``.
 Documented deviations from reference quirks: Q7 (first update used acc+1 micro-batches) and
 Q9/Q10 (throughput accounting) are fixed; Q6 (sampler index ran ahead of consumption) is
 fixed by the loader; the rest of the arithmetic (ceil-based accumulation, step numbering of
@@ -35,7 +36,7 @@ import torch
 from . import models as modeling
 from . import ops
 from .config import BertConfig, batch_arithmetic, overlay_json_config
-from .data import BatchedPretrainingLoader, DistributedSampler, ShardedPretrainingDataset
+from .data import BatchedPretrainingLoader, DistributedSampler, HeldOutSet, ShardedPretrainingDataset
 from .data.tokenization import get_bpe_tokenizer, get_wordpiece_tokenizer
 from .models import BertPretrainingCriterion  # noqa: F401  (public name of run_pretraining.py:96)
 from .models.arena import NO_DECAY_KEYS, ParamArena
@@ -108,6 +109,18 @@ def build_parser() -> argparse.ArgumentParser:
                    help="fused engine: bitwise-reproducible training: the fused engine's fixed-order reductions (no "
                         "floating-point atomics) and torch.use_deterministic_algorithms(True); the same program on the "
                         "same inputs, GPU and build gives the same loss, gradients and weights")
+    # held-out evaluation
+    p.add_argument("--eval_dir", default=None, type=str,
+                   help="file or directory (recursive *.hdf5) of held-out shards: evaluate masked-LM and NSP loss and "
+                        "accuracy on them (off by default)")
+    p.add_argument("--num_eval_examples", type=int, default=10000,
+                   help="size of the held-out set: the first N samples of --eval_dir, masked once with --eval_seed")
+    p.add_argument("--eval_batch_size", type=int, default=None,
+                   help="sequences per evaluation batch and device (default: --local_batch_size)")
+    p.add_argument("--eval_interval", type=int, default=0,
+                   help="evaluate every N optimizer steps and at the end of the session; 0: only at the end")
+    p.add_argument("--eval_seed", type=int, default=0,
+                   help="seed of the held-out set's masks (sample i is masked by a generator seeded from (seed, i))")
     return p
 
 
@@ -318,6 +331,48 @@ def prepare_dataset(args, checkpoint):
     return loader, sampler
 
 
+def prepare_eval_set(args):
+    """The held-out set of ``--eval_dir`` (None without the flag), masked like the training data."""
+    if not getattr(args, "eval_dir", None):
+        return None
+    files = find_input_files(args.eval_dir)
+    if not files:
+        raise ValueError(f"--eval_dir {args.eval_dir} holds no *.hdf5 file")
+    with open(args.model_config_file) as f:
+        cfg = json.load(f)
+    tok = get_wordpiece_tokenizer if cfg.get("tokenizer", "wordpiece") == "wordpiece" else get_bpe_tokenizer
+    tokenizer = tok(cfg["vocab_file"], uppercase=not cfg.get("lowercase", True))
+    eval_set = HeldOutSet(files, args.num_eval_examples, tokenizer.token_to_id("[MASK]"), args.max_predictions_per_seq,
+                          args.masked_token_fraction, cfg["vocab_size"], seed=args.eval_seed,
+                          pin_memory=args.device_obj.type == "cuda")
+    if is_main_process():
+        logger.info(f"Held-out samples: {len(eval_set)}")
+    return eval_set
+
+
+def evaluate(model, eval_set, args) -> Dict[str, float]:
+    """Held-out metrics of the current weights: this rank's slice of ``eval_set``, the six sums all-reduced over the
+    ranks, then the means.  Touches no training state."""
+    base = unwrap(model)
+    device = args.device_obj
+    acc = torch.zeros(6, dtype=torch.float64, device=device)
+    batch_size = args.eval_batch_size or args.local_batch_size
+    fused = base.pretrain_engine() is not None
+    use_amp = not fused and args.compute_dtype in (torch.float16, torch.bfloat16)
+    for batch in eval_set.batches(batch_size, get_rank(), get_world_size()):
+        tokens = packed_tokens(batch[2]) if args.unpad else None
+        batch = [t.to(device, non_blocking=True) for t in batch]
+        with torch.autocast(device_type=device.type, dtype=args.compute_dtype, enabled=use_amp):
+            base.evaluate(*batch, acc, tokens=tokens)
+    model.comm.all_reduce_(acc)
+    s = acc.tolist()
+    out = {"eval_mlm_loss": s[0] / max(s[2], 1.0), "eval_mlm_accuracy": s[1] / max(s[2], 1.0)}
+    if getattr(base.cls, "has_nsp", False):
+        out.update(eval_nsp_loss=s[3] / max(s[5], 1.0), eval_nsp_accuracy=s[4] / max(s[5], 1.0))
+    out["eval_samples"] = len(eval_set)
+    return out
+
+
 # ---------------------------------------------------------------------------
 # step functions
 # ---------------------------------------------------------------------------
@@ -393,6 +448,7 @@ def main(args) -> Tuple[int, float]:
     model, checkpoint, global_step, criterion, args = prepare_model(args)
     optimizer, preconditioner, lr_schedulers, scaler = prepare_optimizers(args, model, checkpoint, global_step)
     loader, sampler = prepare_dataset(args, checkpoint)
+    eval_set = prepare_eval_set(args)
     model.train()
     manager = ckpt_utils.CheckpointManager(args.model_output_dir, keep=3)
     device = args.device_obj
@@ -406,6 +462,18 @@ def main(args) -> Tuple[int, float]:
     timer = DeviceTimer(device)
     train_ms = 0.0
     step_t0 = perf_counter()
+    eval_ms = 0.0                   # evaluation time, kept out of the training time
+    last_eval = None
+
+    def run_eval(step_no: int) -> None:
+        nonlocal eval_ms, last_eval
+        t0 = perf_counter()
+        metrics = evaluate(model, eval_set, args)         # ends in a host read of the sums: the time is complete
+        seconds = perf_counter() - t0
+        eval_ms += seconds * 1e3
+        last_eval = step_no
+        logger.log(tag="eval", step=step_no + args.previous_phase_end_step, **metrics, eval_seconds=seconds)
+
     pbar = None
     if not args.disable_progress_bar and is_main_process():
         from tqdm import tqdm
@@ -491,6 +559,12 @@ def main(args) -> Tuple[int, float]:
             if pbar is not None:
                 pbar.update(1)
             finished = global_step >= args.max_steps or optimization_steps >= args.steps
+            if eval_set is not None and (finished or (args.eval_interval > 0
+                                                      and optimization_steps % args.eval_interval == 0)):
+                run_eval(global_step)
+                clock.reset()                   # the next step's timing starts after the evaluation
+                clock.mark()
+                step_t0 = perf_counter()
             if finished or (optimization_steps % args.num_steps_per_checkpoint == 0):
                 save(global_step)
             if finished:
@@ -500,7 +574,9 @@ def main(args) -> Tuple[int, float]:
             epoch += 1
             continue
         break
-    train_ms = timer.stop()
+    train_ms = timer.stop() - eval_ms
+    if eval_set is not None and last_eval != global_step:
+        run_eval(global_step)           # a session that trained no step still reports the held-out metrics
     if profiler is not None:
         profiler.stop()
     loader.close()

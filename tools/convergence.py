@@ -7,8 +7,10 @@ schedule through three execution paths -- VERDICT r1 #7 / #8:
 
     python tools/convergence.py [--steps 300] [--hidden 1024 --layers 4] > convergence.jsonl
 
-One JSON line per arm with the per-step MLM+NSP loss (dropout off so the three arms see the same function), then a
-summary line with the final-loss ratios (mean of the last 10 % of the steps)."""
+One JSON line per arm with the per-step MLM+NSP loss (dropout off so the three arms see the same function) and the
+held-out masked-LM accuracy and loss at the end of the arm (``BertForPreTraining.evaluate`` on 16 batches drawn from
+a different seed than the training batches), then a summary line with the final-loss ratios (mean of the last 10 % of
+the steps)."""
 import argparse
 import json
 import os
@@ -39,7 +41,7 @@ def batches(n, B, S, V, max_pred, seed):
     return out
 
 
-def run(arm, args, data):
+def run(arm, args, data, heldout):
     torch.manual_seed(1234)
     cfg = BertConfig(vocab_size_or_config_json_file=args.vocab, hidden_size=args.hidden, num_hidden_layers=args.layers,
                      num_attention_heads=args.hidden // 64, intermediate_size=4 * args.hidden,
@@ -75,7 +77,12 @@ def run(arm, args, data):
         opt.step()
         opt.zero_grad()
         losses.append(round(float(loss), 5))
-    return losses
+    acc = torch.zeros(6, dtype=torch.float64, device="cuda")
+    for b in heldout:
+        model.evaluate(*b, acc)
+    s = acc.tolist()
+    return losses, {"heldout_mlm_accuracy": round(s[1] / max(s[2], 1.0), 5),
+                    "heldout_mlm_loss": round(s[0] / max(s[2], 1.0), 5)}
 
 
 def main():
@@ -91,13 +98,14 @@ def main():
     ap.add_argument("--arms", default="oracle-fp32,fused-bf16,fused-fp8")
     args = ap.parse_args()
     data = batches(64, args.batch, args.seq, args.vocab, args.max_pred, seed=7)
+    heldout = batches(16, args.batch, args.seq, args.vocab, args.max_pred, seed=8)
     tail = max(1, args.steps // 10)
     finals = {}
     for arm in args.arms.split(","):
-        losses = run(arm, args, data)
+        losses, held = run(arm, args, data, heldout)
         finals[arm] = sum(losses[-tail:]) / tail
         print(json.dumps({"arm": arm, "config": vars(args), "first_loss": losses[0], "final_loss_mean_last_10pct": round(finals[arm], 5),
-                          "loss": losses}), flush=True)
+                          **held, "loss": losses}), flush=True)
     ref = finals.get("oracle-fp32")
     if ref:
         print(json.dumps({"summary": {a: {"final": round(v, 5), "rel_to_oracle": round(v / ref - 1.0, 5)} for a, v in finals.items()},
