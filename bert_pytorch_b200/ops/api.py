@@ -52,14 +52,15 @@ def _count(n: int = 1) -> None:
     KERNEL_LAUNCHES += n
 
 
-# epilogues that read or write a second [M, N] tensor (residual, GELU' or saved factor, keep bits): on 128 x 128 tiles
-# the kernel runs them ping-pong, under the other warpgroup's MMAs, which measured 5-15 % faster on H100 at the
-# BERT-large shapes than the 128 x 256 tile whose two warpgroups run the epilogue together (tools/gemm_bench.py --epi)
-_HEAVY_EPI = (EPI_BIAS_DROP_RES, EPI_ADD, EPI_BIAS_GELU_DG, EPI_MUL)
+# bias + GELU + GELU' is long enough that on 128 x 128 tiles, where the kernel runs it ping-pong under the other
+# warpgroup's MMAs, it measured 6 % faster on H100 at the BERT-large FFN-1 shape than on the 128 x 256 tile whose two
+# warpgroups run the epilogue together.  The epilogues that read a residual or saved factor stage it through shared
+# memory and measured 1-12 % faster on 128 x 256 tiles (tools/gemm_bench.py --epi).
+_HEAVY_EPI = (EPI_BIAS_GELU_DG,)
 
 
 def _pick_block_n(M: int, N: int, epi: int = EPI_NONE) -> int:
-    """128 for N <= 128 and for the heavy epilogues; otherwise 256 (128 x 256 tiles: half the A-operand traffic per
+    """128 for N <= 128 and for bias + GELU + GELU'; otherwise 256 (128 x 256 tiles: half the A-operand traffic per
     FLOP) unless the narrow tiles waste clearly fewer SM slots in the last wave."""
     if N <= 128 or epi in _HEAVY_EPI:
         return 128

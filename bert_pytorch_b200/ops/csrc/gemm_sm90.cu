@@ -25,7 +25,9 @@
 // with the derivative saved for backward, bias+dropout+residual, residual add, multiply by a saved factor, fp32
 // accumulate-into (wgrad into the gradient arena), bias+tanh, plain fp32.  gemm_bf16 lists the (operand form,
 // epilogue) pairs that are built.  The accumulator fragment is regrouped inside each quad (quad_transpose) so that a
-// thread owns 8 consecutive output columns: one 16-byte store, one Philox draw and one keep-bit byte per group.
+// thread owns 8 consecutive output columns: one 16-byte store, one Philox draw and one keep-bit byte per group.  The
+// bf16 epilogues that read a residual or saved factor, and bias and bias + tanh, stage their output through shared
+// memory and store it with TMA (staged_epilogue); the others store from registers (fragment_epilogue).
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
@@ -49,6 +51,10 @@ struct Cfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = SMEM_BUDGET / STAGE_BYTES;      // 6 (BLOCK_N 128) or 4 (256)
   static constexpr int SMEM_TOTAL = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  // bf16-output epilogues add two 8 KB staging subtiles and a BLOCK_N bias slice per consumer warpgroup (see
+  // staged_epilogue)
+  static constexpr int SMEM_STAGED = SMEM_TOTAL + 2 * (2 * 8192 + BLOCK_N * 2);
+  static_assert(SMEM_STAGED <= 232448, "more dynamic shared memory than an sm_90 block may use");
 };
 
 struct GemmArgs {
@@ -101,101 +107,48 @@ struct UnitStamps {
 #define TL(...)
 #endif
 
-// Epilogue of 8 consecutive output columns [n0, n0 + 8) of one row (n0 % 8 == 0, N % 8 == 0).  `f` holds
-// alpha * accumulator.  Returns through `f` the values that were stored (bf16-rounded) for the column sums.
-template <int E>
-__device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8], int row, int n0, unsigned long long seed,
-                                               bool add_local) {
-  const size_t ooff = (size_t)row * p.ldo + n0;
-  if constexpr (E == EPI_ACCUM_F32) {
-    float* o = reinterpret_cast<float*>(p.out) + ooff;
-    if (p.peer_world > 1) {
-      // an 8-column group crosses at most one shard boundary (shards are multiples of 2048 elements)
-      const long long e0 = p.peer_off + (long long)ooff;
-      const int own0 = (int)min((long long)(p.peer_world - 1), e0 / p.peer_per);
-      const long long bound = own0 + 1 < p.peer_world ? (long long)(own0 + 1) * p.peer_per : (1ll << 62);
-#pragma unroll
-      for (int j = 0; j < 8; j += 4) {
-        const int owner = (e0 + j >= bound) ? own0 + 1 : own0;
-        if (!p.peer_push || owner == p.peer_rank) {
-          asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j), "f"(f[j]),
-                       "f"(f[j + 1]), "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
-        } else {
-          float4 v = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-          if (add_local) {                       // what the earlier micro-steps accumulated here
-            const float4 cur = *reinterpret_cast<const float4*>(o + j);
-            v.x += cur.x; v.y += cur.y; v.z += cur.z; v.w += cur.w;
-          }
-          float* dst = p.peer_base[owner] + (e0 + j);
-          asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y),
-                       "f"(v.z), "f"(v.w) : "memory");
-        }
-      }
-      return;
-    }
-    // fire-and-forget reduction at the L2 (one contributor per element and launch unless split-K)
-#pragma unroll
-    for (int j = 0; j < 8; j += 4)
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j), "f"(f[j]), "f"(f[j + 1]),
-                   "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
-    return;
-  }
-  if constexpr (E == EPI_F32) {
-    float* o = reinterpret_cast<float*>(p.out) + ooff;
-    *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
-    *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
-    return;
-  }
+// bf16-output epilogue math of W consecutive output columns of one row (W even).  `f` holds alpha * accumulator,
+// `bias` and `res` the packed bf16 bias and residual / saved-factor values of those columns (read only when p.bias /
+// p.res is set), `kb` their dropout keep bits (bit t: column t; applied when the epilogue drops).  Writes the packed
+// bf16 output to `out` and, for EPI_BIAS_GELU_DG, gelu' to `aux`.
+template <int E, int W>
+__device__ __forceinline__ void epilogue_math(const GemmArgs& p, float (&f)[W], const uint32_t (&bias)[W / 2],
+                                              uint32_t kb, const uint32_t (&res)[W / 2], uint32_t (&out)[W / 2],
+                                              uint32_t (&aux)[W / 2]) {
   if constexpr (epilogue_spec(E).bias) {
     if (p.bias != nullptr) {
-      const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + n0));
-      const uint32_t w[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float2 bb = unpack_bf16(w[t]);
+      for (int t = 0; t < W / 2; ++t) {
+        const float2 bb = unpack_bf16(bias[t]);
         f[2 * t] += bb.x;
         f[2 * t + 1] += bb.y;
       }
     }
   }
   if constexpr (E == EPI_BIAS_GELU_DG) {
-    float dg[8];
+    float dg[W];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+    for (int j = 0; j < W; ++j) {
       const GeluParts gp = gelu_parts(f[j]);
       dg[j] = fmaf(f[j] * 0.3989422804014327f, gp.e, gp.Phi);
       f[j] *= gp.Phi;
     }
-    *reinterpret_cast<uint4*>(p.aux_out + ooff) =
-        make_uint4(pack_bf16(dg[0], dg[1]), pack_bf16(dg[2], dg[3]), pack_bf16(dg[4], dg[5]), pack_bf16(dg[6], dg[7]));
+#pragma unroll
+    for (int t = 0; t < W / 2; ++t) aux[t] = pack_bf16(dg[2 * t], dg[2 * t + 1]);
   } else if constexpr (E == EPI_BIAS_TANH) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) f[j] = tanhf(f[j]);
+    for (int j = 0; j < W; ++j) f[j] = tanhf(f[j]);
   } else if constexpr (E == EPI_BIAS_DROP_RES || E == EPI_ADD || E == EPI_MUL) {
     if constexpr (epilogue_spec(E).keep_bits) {
       if (p.drop_thresh16 != 0) {
-        const size_t moff = (size_t)row * (size_t)(p.N >> 3) + (size_t)(n0 >> 3);
-        uint32_t kb;
-        if (p.mask_in != nullptr) {
-          kb = __ldg(p.mask_in + moff);
-        } else {
-          const uint64_t e8 = ((uint64_t)row * (uint64_t)p.N + (uint64_t)n0) >> 3;
-          const Keep8 keep = dropout_keep8(seed, p.stream, e8, p.drop_thresh16);
-          kb = 0;
 #pragma unroll
-          for (int t = 0; t < 8; ++t) kb |= (keep[t] ? 1u : 0u) << t;
-          if (p.mask_out != nullptr) p.mask_out[moff] = (unsigned char)kb;
-        }
-#pragma unroll
-        for (int t = 0; t < 8; ++t) f[t] = (kb >> t) & 1u ? __fmul_rn(f[t], p.drop_scale) : 0.f;
+        for (int t = 0; t < W; ++t) f[t] = (kb >> t) & 1u ? __fmul_rn(f[t], p.drop_scale) : 0.f;
       }
     }
     if (p.res != nullptr) {
-      const uint4 r = *reinterpret_cast<const uint4*>(p.res + (size_t)row * p.ldr + n0);
-      const uint32_t w[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float2 rr = unpack_bf16(w[t]);
+      for (int t = 0; t < W / 2; ++t) {
+        const float2 rr = unpack_bf16(res[t]);
         if constexpr (E == EPI_MUL) {
           f[2 * t] *= rr.x;
           f[2 * t + 1] *= rr.y;
@@ -206,15 +159,8 @@ __device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8],
       }
     }
   }
-  const uint4 o = make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + ooff) = o;
-  const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    const float2 v = unpack_bf16(ow[t]);
-    f[2 * t] = v.x;
-    f[2 * t + 1] = v.y;
-  }
+  for (int t = 0; t < W / 2; ++t) out[t] = pack_bf16(f[2 * t], f[2 * t + 1]);
 }
 
 // Work unit u of a launch: output tile (mb, nb) and k-blocks [kb0, kb0 + nkb) -- split-major, then m-block, then
@@ -286,10 +232,91 @@ __device__ __forceinline__ void consumer_mainloop(float (&acc)[R][BLOCK_N / 2], 
   if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
 }
 
-// Epilogue of one warpgroup's 64 x NCOLS accumulator fragment: output rows [row64, row64 + 64), columns from col0.
+// Register epilogue of 8 consecutive output columns [n0, n0 + 8) of one row (n0 % 8 == 0, N % 8 == 0), stored
+// straight from registers (the epilogues that do not stage their output, see staged_epi).  `f` holds alpha *
+// accumulator.  Returns through `f` the values that were stored (bf16-rounded) for the column sums.
+template <int E>
+__device__ __forceinline__ void epilogue_group(const GemmArgs& p, float (&f)[8], int row, int n0, bool add_local) {
+  const size_t ooff = (size_t)row * p.ldo + n0;
+  if constexpr (E == EPI_ACCUM_F32) {
+    float* o = reinterpret_cast<float*>(p.out) + ooff;
+    if (p.peer_world > 1) {
+      // an 8-column group crosses at most one shard boundary (shards are multiples of 2048 elements)
+      const long long e0 = p.peer_off + (long long)ooff;
+      const int own0 = (int)min((long long)(p.peer_world - 1), e0 / p.peer_per);
+      const long long bound = own0 + 1 < p.peer_world ? (long long)(own0 + 1) * p.peer_per : (1ll << 62);
+#pragma unroll
+      for (int j = 0; j < 8; j += 4) {
+        const int owner = (e0 + j >= bound) ? own0 + 1 : own0;
+        if (!p.peer_push || owner == p.peer_rank) {
+          asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j), "f"(f[j]),
+                       "f"(f[j + 1]), "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
+        } else {
+          float4 v = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
+          if (add_local) {                       // what the earlier micro-steps accumulated here
+            const float4 cur = *reinterpret_cast<const float4*>(o + j);
+            v.x += cur.x; v.y += cur.y; v.z += cur.z; v.w += cur.w;
+          }
+          float* dst = p.peer_base[owner] + (e0 + j);
+          asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y),
+                       "f"(v.z), "f"(v.w) : "memory");
+        }
+      }
+      return;
+    }
+    // fire-and-forget reduction at the L2 (one contributor per element and launch unless split-K)
+#pragma unroll
+    for (int j = 0; j < 8; j += 4)
+      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(o + j), "f"(f[j]), "f"(f[j + 1]),
+                   "f"(f[j + 2]), "f"(f[j + 3]) : "memory");
+    return;
+  }
+  if constexpr (E == EPI_F32) {
+    float* o = reinterpret_cast<float*>(p.out) + ooff;
+    *reinterpret_cast<float4*>(o) = make_float4(f[0], f[1], f[2], f[3]);
+    *reinterpret_cast<float4*>(o + 4) = make_float4(f[4], f[5], f[6], f[7]);
+    return;
+  }
+  uint32_t bias[4] = {0, 0, 0, 0}, ow[4], aux[4];
+  const uint32_t none[4] = {0, 0, 0, 0};
+  if constexpr (epilogue_spec(E).bias) {
+    if (p.bias != nullptr) {
+      const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.bias + n0));
+      bias[0] = b.x; bias[1] = b.y; bias[2] = b.z; bias[3] = b.w;
+    }
+  }
+  epilogue_math<E, 8>(p, f, bias, 0, none, ow, aux);
+  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + ooff) = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+  if constexpr (epilogue_spec(E).aux)
+    *reinterpret_cast<uint4*>(p.aux_out + ooff) = make_uint4(aux[0], aux[1], aux[2], aux[3]);
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const float2 v = unpack_bf16(ow[t]);
+    f[2 * t] = v.x;
+    f[2 * t + 1] = v.y;
+  }
+}
+
+// Accumulator values of 8 output columns of one row after the quad regrouping: 32-column chunk i of the fragment,
+// row half h, as alpha * acc.  __fmul_rn: alpha * acc is rounded to fp32 before the bias or residual add that follows,
+// so that add is never contracted into an fma.  The outputs are defined with that rounding.
+__device__ __forceinline__ void regroup8(float (&f)[8], const uint32_t (&lo_in)[4], const uint32_t (&hi_in)[4],
+                                         float alpha) {
+  uint32_t lo[4] = {lo_in[0], lo_in[1], lo_in[2], lo_in[3]}, hi[4] = {hi_in[0], hi_in[1], hi_in[2], hi_in[3]};
+  quad_transpose(lo);
+  quad_transpose(hi);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    f[2 * k] = __fmul_rn(__uint_as_float(lo[k]), alpha);
+    f[2 * k + 1] = __fmul_rn(__uint_as_float(hi[k]), alpha);
+  }
+}
+
+// Register epilogue of one warpgroup's 64 x NCOLS accumulator fragment: output rows [row64, row64 + 64), columns from
+// col0.
 template <int NCOLS, int E>
 __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc)[NCOLS / 2], int row64, int col0,
-                                                  float alpha, unsigned long long seed, bool add_local) {
+                                                  float alpha, bool add_local) {
   const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
   const int c = lane & 3;
   const int row_base = row64 + warp * 16 + (lane >> 2);
@@ -308,24 +335,16 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
         lo[k] = __float_as_uint(acc[(i * 4 + k) * 4 + 2 * h]);
         hi[k] = __float_as_uint(acc[(i * 4 + k) * 4 + 2 * h + 1]);
       }
-      quad_transpose(lo);
-      quad_transpose(hi);
+      float f[8];
+      regroup8(f, lo, hi, alpha);
       const int row = row_base + h * 8;
       if (row < p.M && n0 < p.N) {
-        float f[8];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          // __fmul_rn: alpha * acc is rounded to fp32 before the bias or residual add that follows, so that add is
-          // never contracted into an fma.  The outputs are defined with that rounding.
-          f[2 * k] = __fmul_rn(__uint_as_float(lo[k]), alpha);
-          f[2 * k + 1] = __fmul_rn(__uint_as_float(hi[k]), alpha);
-        }
-        epilogue_group<E>(p, f, row, n0, seed, add_local);
+        epilogue_group<E>(p, f, row, n0, add_local);
 #pragma unroll
         for (int t = 0; t < 8; ++t) cs[t] += f[t];
       }
     }
-    if constexpr (!epilogue_spec(E).f32_out) {
+    if constexpr (epilogue_spec(E).colsum) {
       if (p.colsum != nullptr) {                 // bias gradients: rows of this warp, then one atomic per column
 #pragma unroll
         for (int t = 0; t < 8; ++t) {
@@ -342,19 +361,223 @@ __device__ __forceinline__ void fragment_epilogue(const GemmArgs& p, float (&acc
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// bf16-output epilogue through shared memory.  Each consumer warpgroup owns two 8 KB staging buffers, each one 64 x 64
+// bf16 subtile with 128-byte rows in the SWIZZLE_128B layout of a [64][64] tensor-map box.  Per subtile the warpgroup
+// converts its accumulator fragment, reads its residual / saved factor from the buffer (loaded by TMA, ahead of use),
+// writes the output to the same addresses, and one thread stores the buffer with a TMA bulk store.  TMA clips the
+// ragged M / N edges, so nothing outside the [M, N] window is written.
+// ---------------------------------------------------------------------------------------------------------------------
+// Which epilogues stage their output.  The plain store (EPI_NONE) and bias + GELU + GELU' (EPI_BIAS_GELU_DG) read no
+// [M, N] input and measured faster on H100 with their stores issued straight from registers; the fp32 outputs are
+// reductions or plain stores that need no staging.
+__host__ __device__ constexpr bool staged_epi(int E) { return !epilogue_spec(E).f32_out && E != EPI_NONE && E != EPI_BIAS_GELU_DG; }
+
+constexpr int SUB_BYTES = 64 * 128;
+constexpr int STAGE_BUFS = 2;                   // per consumer warpgroup
+
+// byte offset of 16-byte chunk `chunk` (0..7) of row `row` in a swizzled subtile
+__device__ __forceinline__ uint32_t sw128(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
+
+// the 128 threads of consumer warpgroup cw (named barriers 1 and 2 are the ping-pong turn barriers).  Not the .aligned
+// form (bar.sync): the thread that issues the bulk copies reaches it from its own branch and mbarrier wait loop.
+__device__ __forceinline__ void wg_sync(int cw) { asm volatile("barrier.sync %0, 128;" ::"r"(3 + cw) : "memory"); }
+
+// Where a warpgroup's bf16 epilogue runs in a unit: its `nsub` 64-column subtiles hold output columns and its `rlive`
+// 64-row fragments hold output rows.  Subtile t = s * rlive + r uses staging buffer (q + t) & 1, where q counts the
+// subtiles the warpgroup staged in its earlier units.
+struct StagedUnit {
+  int row64, col0, nsub, rlive;
+  uint32_t q;
+  __device__ int count() const { return nsub * rlive; }
+};
+
+template <int BLOCK_N, int R>
+__device__ __forceinline__ StagedUnit staged_unit(const GemmArgs& p, int row64, int nb, uint32_t q) {
+  StagedUnit su;
+  su.row64 = row64;
+  su.col0 = nb * BLOCK_N;
+  su.nsub = (min(BLOCK_N, p.N - su.col0) + 63) / 64;
+  const int rows_left = p.M - row64;
+  su.rlive = rows_left <= 0 ? 0 : (R == 2 && rows_left > 64 ? 2 : 1);
+  su.q = q;
+  return su;
+}
+
+// staging buffers and their load barriers (one per buffer) of consumer warpgroup cw
+template <int BLOCK_N>
+__device__ __forceinline__ uint8_t* staging(uint8_t* smem, int cw) {
+  return smem + Cfg<BLOCK_N>::STAGES * Cfg<BLOCK_N>::STAGE_BYTES + cw * STAGE_BUFS * SUB_BYTES;
+}
+template <int BLOCK_N>
+__device__ __forceinline__ uint64_t* in_bars(uint8_t* smem, int cw) {
+  return reinterpret_cast<uint64_t*>(staging<BLOCK_N>(smem, 2)) + 2 * Cfg<BLOCK_N>::STAGES + cw * STAGE_BUFS;
+}
+
+// bias slice of consumer warpgroup cw's unit, after the barriers
+template <int BLOCK_N>
+__device__ __forceinline__ uint32_t bias_slice(uint8_t* smem, int cw) {
+  return smem_u32(staging<BLOCK_N>(smem, 2) + 256) + cw * BLOCK_N * 2;
+}
+
+// TMA load of the residual / saved factor of subtile t = s * rlive + r into its staging buffer
+__device__ __forceinline__ void load_input(const CUtensorMap* tm_res, uint8_t* buf, uint64_t* in_bar,
+                                           const StagedUnit& su, int t, int s, int r) {
+  const uint32_t b = (su.q + t) & 1;
+  mbar_arrive_expect_tx(&in_bar[b], SUB_BYTES);
+  tma_load_2d(buf + b * SUB_BYTES, tm_res, &in_bar[b], su.col0 + s * 64, su.row64 + r * 64);
+}
+
+template <int BLOCK_N, int R, int E>
+__device__ __forceinline__ void staged_epilogue(const GemmArgs& p, float (&acc)[R][BLOCK_N / 2], const CUtensorMap* tm_out,
+                                                const CUtensorMap* tm_res, uint8_t* smem,
+                                                const StagedUnit& su, int cw, float alpha, unsigned long long seed,
+                                                const uint32_t (&kwords)[R][2][BLOCK_N / 128]) {
+  constexpr EpilogueSpec SP = epilogue_spec(E);
+  int tid = threadIdx.x & 127;
+  asm volatile("" : "+r"(tid));    // derived addresses are recomputed per unit, not held across the main loop
+  const int lane = tid & 31, warp = tid >> 5, c = lane & 3;
+  const bool issuer = tid == 0;
+  const bool has_in = (SP.res || E == EPI_ADD) && p.res != nullptr;   // residual or saved factor, loaded by TMA
+  uint8_t* buf = staging<BLOCK_N>(smem, cw);
+  uint64_t* in_bar = in_bars<BLOCK_N>(smem, cw);
+  const uint32_t buf_s = smem_u32(buf);
+  const int n_staged = su.count();
+  const uint32_t bias_s = bias_slice<BLOCK_N>(smem, cw);
+  if constexpr (SP.bias) {                       // the unit's bias slice, copied in before the main loop
+    if (p.bias != nullptr) {
+      asm volatile("cp.async.wait_all;" ::: "memory");
+      wg_sync(cw);
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < BLOCK_N / 64; ++s) {
+    if (s >= su.nsub) break;                                   // warpgroup uniform
+    float cs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (r >= su.rlive) break;                                // warpgroup uniform
+      const int t = s * su.rlive + r;
+      const uint32_t b = (su.q + t) & 1;
+      const uint32_t sub = buf_s + b * SUB_BYTES;
+      if (has_in) mbar_wait_mma(&in_bar[b], ((su.q + t) >> 1) & 1);
+      // The accumulator is used in its wgmma layout: this lane owns columns 8 j + 2 c, + 1 of each 8-column group j,
+      // rows rr and rr + 8.  Its 4-byte reads and writes of a row's group sit in 16-byte chunk j, which the swizzle
+      // spreads over the 8 rows of the warp: no bank conflicts.
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int rr = warp * 16 + (lane >> 2) + h * 8;        // row inside the subtile
+        const int row = su.row64 + r * 64 + rr;
+        // keep bits drawn here (no mask_in): lane c draws groups c and 4 + c of the row, one Philox evaluation per
+        // group as before, and the quad shares the bytes
+        uint32_t kq[2] = {0, 0};
+        if constexpr (SP.keep_bits) {
+          if (p.drop_thresh16 != 0 && p.mask_in == nullptr) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int n0 = su.col0 + s * 64 + (4 * e + c) * 8;
+              const Keep8 keep =
+                  dropout_keep8(seed, p.stream, ((uint64_t)row * (uint64_t)p.N + (uint64_t)n0) >> 3, p.drop_thresh16);
+#pragma unroll
+              for (int t = 0; t < 8; ++t) kq[e] |= (keep[t] ? 1u : 0u) << t;
+              if (p.mask_out != nullptr && row < p.M && n0 < p.N)
+                p.mask_out[(size_t)row * (size_t)(p.N >> 3) + (size_t)(n0 >> 3)] = (unsigned char)kq[e];
+            }
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int jb = s * 8 + j;                            // 8-column group of the fragment
+          float f[2] = {__fmul_rn(acc[r][jb * 4 + 2 * h], alpha), __fmul_rn(acc[r][jb * 4 + 2 * h + 1], alpha)};
+          const uint32_t addr = sub + sw128(rr, j) + c * 4;
+          uint32_t res[1] = {0}, bias[1] = {0}, out[1], aux[1];
+          if (has_in) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(res[0]) : "r"(addr) : "memory");
+          if constexpr (SP.bias)
+            if (p.bias != nullptr)
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(bias[0]) : "r"(bias_s + (jb * 8 + c * 2) * 2) : "memory");
+          uint32_t kb = 0;
+          if constexpr (SP.keep_bits) {
+            if (p.drop_thresh16 != 0) {
+              // keep byte of group jb: from mask_in, byte jb % 16 of the row's 16 bytes of 128-column chunk jb / 16,
+              // held in word (jb % 16) / 4 by that quad lane; or drawn above by lane j % 4
+              const uint32_t byte =
+                  p.mask_in != nullptr
+                      ? __shfl_sync(0xffffffffu, kwords[r][h][jb >> 4], (lane & ~3) | ((jb & 15) >> 2)) >> (8 * (jb & 3))
+                      : __shfl_sync(0xffffffffu, kq[j >> 2], (lane & ~3) | (j & 3));
+              kb = (byte >> (2 * c)) & 3u;
+            }
+          }
+          epilogue_math<E, 2>(p, f, bias, kb, res, out, aux);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(out[0]) : "memory");
+        }
+      }
+      fence_proxy_async();                                     // the generic-proxy writes -> the TMA store
+      if (issuer) tma_store_wait_read<0>();                    // the other buffer is free once this barrier is passed
+      wg_sync(cw);
+      if (issuer) {
+        tma_store_2d(tm_out, buf + b * SUB_BYTES, su.col0 + s * 64, su.row64 + r * 64);
+        tma_store_commit();
+      }
+      if constexpr (SP.colsum) {
+        if (p.colsum != nullptr) {
+          // column pair cp of the subtile, rows 16 qd .. 16 qd + 15 in a rotated order (conflict-free reads)
+          int l2 = lane;
+          asm volatile("" : "+r"(l2));
+          const int cp = warp * 8 + (l2 & 7), qd = l2 >> 3;
+#pragma unroll 1
+          for (int j = 0; j < 16; ++j) {
+            const int rs = 16 * qd + ((j + 2 * qd) & 15);
+            uint32_t v;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(sub + sw128(rs, cp >> 2) + (cp & 3) * 4) : "memory");
+            if (su.row64 + r * 64 + rs < p.M) {
+              const float2 x = unpack_bf16(v);
+              cs[0] += x.x;
+              cs[1] += x.y;
+            }
+          }
+          if (has_in) wg_sync(cw);                             // every read of the buffer is done before it is reloaded
+        }
+      }
+      if (has_in && issuer && t + 2 < n_staged) {
+        tma_store_wait_read<0>();
+        if (su.rlive == 2) load_input(tm_res, buf, in_bar, su, t + 2, s + 1, r);
+        else load_input(tm_res, buf, in_bar, su, t + 2, s + 2, 0);
+      }
+    }
+    if constexpr (SP.colsum) {
+      if (p.colsum != nullptr) {                 // bias gradients: one atomic per column, subtile and warpgroup
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          cs[e] += __shfl_xor_sync(0xffffffffu, cs[e], 8);
+          cs[e] += __shfl_xor_sync(0xffffffffu, cs[e], 16);
+        }
+        const int n = su.col0 + s * 64 + 2 * (warp * 8 + (lane & 7));
+        if (lane < 8 && n < p.N) {
+          atomicAdd(p.colsum + n, cs[0]);
+          atomicAdd(p.colsum + n + 1, cs[1]);
+        }
+      }
+    }
+  }
+}
+
 // The consumer warpgroup `cw` (0 or 1) over this CTA's units.  Ping-pong (BLOCK_N 128): warpgroup cw takes the
 // CTA's units j = cw, cw + 2, ...; it waits on named barrier 1 + cw for its turn to issue MMAs and, if the other
 // warpgroup has a next unit, hands the turn over on barrier 2 - cw once its own MMAs are issued.  The order also keeps
 // a warpgroup from running more than one ring phase ahead of the producer.
 template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int AE5, int BE5, int E>
-__device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
-                                         int cw) {
+__device__ __forceinline__ void consumer(const GemmArgs& p, const CUtensorMap* tm_out, const CUtensorMap* tm_res,
+                                         uint8_t* smem, uint64_t* full_bar,
+                                         uint64_t* empty_bar, int cw) {
   constexpr bool PINGPONG = BLOCK_N == 128;
   constexpr int R = PINGPONG ? 2 : 1;            // 64-row accumulator fragments per warpgroup
+  constexpr EpilogueSpec SP = epilogue_spec(E);
   float acc[R][BLOCK_N / 2];                     // the first MMA of a unit overwrites it (scale-d = 0)
   float alpha = p.alpha;
   if constexpr (FP8) alpha *= __ldg(p.scale_a) * __ldg(p.scale_b);   // per-tensor dequantisation
   const unsigned long long seed = p.drop_thresh16 != 0 ? p.seed.value() : 0ull;
+  const bool issuer = (threadIdx.x & 127) == 0;  // issues this warpgroup's TMA loads and stores
+  uint32_t q = 0;                                // subtiles this warpgroup has staged
   if (PINGPONG && cw == 1) asm volatile("bar.arrive 1, 256;" ::: "memory");   // warpgroup 0 goes first
   uint32_t it = 0;                               // ring position of the unit: k-blocks of this CTA's earlier units
   int j = 0;
@@ -366,14 +589,60 @@ __device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint6
     }
     if (PINGPONG) asm volatile("bar.sync %0, 256;" ::"r"(1 + cw) : "memory");
     TL(UnitStamps st{}; st.start = clock64();)
+    const int row64 = w.mb * BLOCK_M + (PINGPONG ? 0 : cw * 64);
+    if constexpr (staged_epi(E)) {
+      if (issuer && p.res != nullptr && (SP.res || E == EPI_ADD)) {   // the first two subtiles land under the MMAs
+        const StagedUnit su = staged_unit<BLOCK_N, R>(p, row64, w.nb, q);
+        tma_store_wait_read<0>();
+        uint8_t* buf = staging<BLOCK_N>(smem, cw);
+        uint64_t* in_bar = in_bars<BLOCK_N>(smem, cw);
+        if (su.count() > 0) load_input(tm_res, buf, in_bar, su, 0, 0, 0);
+        if (su.count() > 1) load_input(tm_res, buf, in_bar, su, 1, su.rlive == 2 ? 0 : 1, su.rlive == 2 ? 1 : 0);
+      }
+    }
+    // the unit's bias slice goes to shared memory and its mask_in keep bytes to registers while the MMAs run: for each
+    // of the thread's rows and 128-column chunks, word c of the row's 16 keep bytes (the quad shares them)
+    uint32_t kwords[R][2][BLOCK_N / 128];
+    if constexpr (staged_epi(E)) {
+      const int tid = threadIdx.x & 127;
+      if constexpr (SP.bias) {
+        const int n = w.nb * BLOCK_N + tid * 2;
+        if (p.bias != nullptr && tid < BLOCK_N / 2)
+          asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(bias_slice<BLOCK_N>(smem, cw) + tid * 4),
+                       "l"(p.bias + (n < p.N ? n : 0)), "r"(n < p.N ? 4 : 0) : "memory");
+      }
+      if constexpr (SP.keep_bits) {
+        if (p.drop_thresh16 != 0 && p.mask_in != nullptr) {
+#pragma unroll
+          for (int r = 0; r < R; ++r)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row64 + r * 64 + (tid >> 5) * 16 + ((tid & 31) >> 2) + h * 8;
+#pragma unroll
+              for (int x = 0; x < BLOCK_N / 128; ++x) {
+                const int n = w.nb * BLOCK_N + x * 128;
+                kwords[r][h][x] =
+                    row < p.M && n < p.N
+                        ? __ldg(reinterpret_cast<const uint32_t*>(p.mask_in + (size_t)row * (p.N >> 3) + (n >> 3)) + (tid & 3))
+                        : 0u;
+              }
+            }
+        }
+      }
+    }
     const int arrive_bar = PINGPONG && u + (int)gridDim.x < p.units ? 2 - cw : -1;
     consumer_mainloop<A_MN, B_MN, BLOCK_N, R, FP8, AE5, BE5>(acc, smem, full_bar, empty_bar, PINGPONG ? 0 : cw, it,
                                                             w.nkb, arrive_bar TL(, st));
     it += w.nkb;
-    const int row64 = w.mb * BLOCK_M + (PINGPONG ? 0 : cw * 64);
+    if constexpr (!staged_epi(E)) {
 #pragma unroll
-    for (int r = 0; r < R; ++r)
-      fragment_epilogue<BLOCK_N, E>(p, acc[r], row64 + r * 64, w.nb * BLOCK_N, alpha, seed, w.ks == 0);
+      for (int r = 0; r < R; ++r)
+        fragment_epilogue<BLOCK_N, E>(p, acc[r], row64 + r * 64, w.nb * BLOCK_N, alpha, w.ks == 0);
+    } else {
+      const StagedUnit su = staged_unit<BLOCK_N, R>(p, row64, w.nb, q);
+      staged_epilogue<BLOCK_N, R, E>(p, acc, tm_out, tm_res, smem, su, cw, alpha, seed, kwords);
+      q += su.count();
+    }
 #ifdef B200_GEMM_TIMELINE
     st.epi_done = clock64();
     if (p.timeline != nullptr && (threadIdx.x & 127) == 0) {
@@ -383,19 +652,24 @@ __device__ __forceinline__ void consumer(const GemmArgs& p, uint8_t* smem, uint6
     }
 #endif
   }
+  if (staged_epi(E) && issuer) tma_store_wait<0>();   // the bulk stores have read the staging buffers before exit
 }
 
 // E: the epilogue (GemmEpilogue), see epilogue_group
 template <bool A_MN, bool B_MN, int BLOCK_N, bool FP8, int E>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res,
             const GemmArgs p) {
   using C = Cfg<BLOCK_N>;
   static_assert(!FP8 || (!A_MN && !B_MN), "fp8 wgmma reads K-major operands only");
+  constexpr bool STAGED = staged_epi(E);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
+  // operand ring, then (bf16 epilogues) the staging subtiles, then full_bar, empty_bar and in_bar
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging<BLOCK_N>(smem, 0) + (STAGED ? 2 * STAGE_BUFS * SUB_BYTES : 0));
   uint64_t* empty_bar = full_bar + C::STAGES;
+  uint64_t* in_bar = in_bars<BLOCK_N>(smem, 0);
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
@@ -405,6 +679,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], BLOCK_N == 128 ? 4 : 8);   // one arrival per warp of the warpgroup(s) reading the slot
     }
+    if (STAGED)
+      for (int b = 0; b < 2 * STAGE_BUFS; ++b) mbar_init(&in_bar[b], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -459,13 +735,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   const int cw = wg - 1;
   if constexpr (FP8) {
     switch (p.fp8_fmt & 3u) {
-      case 0: consumer<A_MN, B_MN, BLOCK_N, true, 0, 0, E>(p, smem, full_bar, empty_bar, cw); break;
-      case 1: consumer<A_MN, B_MN, BLOCK_N, true, 1, 0, E>(p, smem, full_bar, empty_bar, cw); break;
-      case 2: consumer<A_MN, B_MN, BLOCK_N, true, 0, 1, E>(p, smem, full_bar, empty_bar, cw); break;
-      default: consumer<A_MN, B_MN, BLOCK_N, true, 1, 1, E>(p, smem, full_bar, empty_bar, cw); break;
+      case 0: consumer<A_MN, B_MN, BLOCK_N, true, 0, 0, E>(p, &tmap_out, &tmap_res, smem, full_bar, empty_bar, cw); break;
+      case 1: consumer<A_MN, B_MN, BLOCK_N, true, 1, 0, E>(p, &tmap_out, &tmap_res, smem, full_bar, empty_bar, cw); break;
+      case 2: consumer<A_MN, B_MN, BLOCK_N, true, 0, 1, E>(p, &tmap_out, &tmap_res, smem, full_bar, empty_bar, cw); break;
+      default: consumer<A_MN, B_MN, BLOCK_N, true, 1, 1, E>(p, &tmap_out, &tmap_res, smem, full_bar, empty_bar, cw); break;
     }
   } else {
-    consumer<A_MN, B_MN, BLOCK_N, false, 0, 0, E>(p, smem, full_bar, empty_bar, cw);
+    consumer<A_MN, B_MN, BLOCK_N, false, 0, 0, E>(p, &tmap_out, &tmap_res, smem, full_bar, empty_bar, cw);
   }
 }
 
@@ -617,10 +893,16 @@ static void launch(const GemmCall& c, cudaStream_t st) {
                         : make_tmap_2d(c.A, c.K, c.M, c.lda, BK, 64 * 2, ES);
   CUtensorMap tb = B_MN ? make_tmap_2d(c.B, c.N, c.K, c.ldb, 64, BK, ES)
                         : make_tmap_2d(c.B, c.K, c.N, c.ldb, BK, BLOCK_N, ES);
+  // out and res of the bf16 epilogues: box [64][64], dims [M, N] and the tensor's own row stride, so TMA clips the
+  // ragged edges and never touches a column past N of a wider tensor
+  constexpr bool STAGED = staged_epi(E);
+  const CUtensorMap to = STAGED ? make_tmap_2d(c.out, c.N, c.M, c.ldo, 64, 64, 2) : ta;
+  const CUtensorMap tres = STAGED && c.res != nullptr ? make_tmap_2d(c.res, c.N, c.M, c.ldr, 64, 64, 2) : to;
+  constexpr int SMEM = STAGED ? C::SMEM_STAGED : C::SMEM_TOTAL;
   auto kern = gemm_kernel<A_MN, B_MN, BLOCK_N, FP8, E>;
   static bool configured = false;
   if (!configured) {
-    B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_TOTAL));
+    B200_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     configured = true;
   }
   p.units = p.m_blocks * p.n_blocks * p.k_splits;
@@ -628,7 +910,7 @@ static void launch(const GemmCall& c, cudaStream_t st) {
   p.timeline = p.units <= g_timeline_units ? g_timeline : nullptr;
 #endif
   const int grid = p.units < num_sms() ? p.units : num_sms();       // persistent: one CTA per SM walks the units
-  launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_TOTAL, st, ta, tb, p);
+  launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), SMEM, st, ta, tb, to, tres, p);
 }
 
 // fp8: bring an MN-major operand ([K][ld], the M or N index contiguous) into the K-major form [MN][Kp]
