@@ -53,10 +53,16 @@ from .arena import ParamArena
 # dropout stream ids: stream = layer * 8 + site
 SITE_EMB, SITE_ATTN_PROB, SITE_ATTN_OUT, SITE_FFN_OUT = 0, 1, 2, 3
 _EMB_LAYER = 1023
+# dropout on the pooled row of the sequence classifier (FusedClassifier): site 4 of the embedding's layer slot.  No
+# encoder layer uses site 4 and the embedding uses site 0, so the stream collides with none of theirs at any depth.
+SITE_CLS = 4
 
 
 def _stream(layer: int, site: int) -> int:
     return layer * 8 + site
+
+
+CLS_STREAM = _stream(_EMB_LAYER, SITE_CLS)
 
 
 def _as_tuple(x):
@@ -709,42 +715,22 @@ def head_linear(linear: torch.nn.Linear, x: torch.Tensor) -> torch.Tensor:
     return linear(x)
 
 
-class FusedPretrainer:
-    """Forward + backward of ``BertForPreTraining`` + criterion as one kernel program.
-
-    ``forward_backward`` returns the (unscaled) loss of the micro-batch as a device scalar and leaves the
-    gradients -- multiplied by ``grad_scale`` (= loss_scale / accumulation_steps) -- accumulated in the arena.
-    """
+class _GraphedProgram:
+    """What the fused training programs share: the token bucket of an unpadded batch, and the policy that runs a
+    kernel program eagerly for its first ``graph_warmup`` calls per input signature, then captures it once and replays
+    it as one CUDA graph, every capture in one memory pool."""
 
     def __init__(self, model):
         self.model = model
         self.engine: FusedEncoderEngine = model.bert.fused_engine()
         self.arena = self.engine.arena
-        cfg = model.config
-        self.V, self.H = cfg.vocab_size, cfg.hidden_size
-        self.has_nsp = model.cls.has_nsp and model.bert.pooler is not None
-        self.max_pred = int(getattr(cfg, "max_predictions_per_seq", 0)) or None
-        self._loss = None
         # CUDA graphs: the micro-step is ~600 launches of static shape; replaying it as one graph removes the
         # launch gaps (~6 % of the phase-1 step).  B200_GRAPH=0 keeps the eager program.
         self.use_graphs = os.environ.get("B200_GRAPH", "1") != "0"
         self.graph_warmup = 2                 # eager calls per input signature before capturing
         self._graphs: Dict[tuple, dict] = {}
         self._seed_step: Optional[torch.Tensor] = None
-        self.grad_push = False                # set by the runtime around the last micro-step (PeerComm.begin_push)
-        self._cls_idx = None                  # row indices of the [CLS] tokens (NSP head)
         self._cap_stream = None               # high-priority capture stream (wgrad side-stream mode)
-        self._cls_S = 0
-        self._eval_cls: Dict[tuple, torch.Tensor] = {}   # [CLS] row indices of the evaluation batch shapes
-
-    def _max_pred(self, labels: torch.Tensor) -> int:
-        # capacity of masked positions per sequence; fixed per run so shapes stay static
-        if self.max_pred is None:
-            # no --max_predictions_per_seq: the capacity is the sequence length (any batch fits; the static-shape head
-            # then costs S rows per sequence, so runners should always pass the flag -- data/dataset.py validates
-            # pre-masked shards against it)
-            self.max_pred = (labels.size(1) + 7) // 8 * 8
-        return self.max_pred
 
     def _graph_ok(self) -> bool:
         kf = getattr(self.model.bert, "_kfac", None)
@@ -762,8 +748,8 @@ class FusedPretrainer:
         eng = self.engine
         if eng.fp8 or _use_sdpa():
             if not getattr(self, "_unpad_warned", False):
-                warnings.warn("BertModel.unpad: fp8 operands and B200_ATTN=sdpa have no unpadded pre-training path; "
-                              "running padded")
+                warnings.warn("BertModel.unpad: fp8 operands and B200_ATTN=sdpa have no unpadded pre-training path or "
+                              "classification program; running padded")
                 self._unpad_warned = True
             return None
         kf = getattr(self.model.bert, "_kfac", None)
@@ -771,6 +757,114 @@ class FusedPretrainer:
             return None
         B, S = input_mask.shape
         return token_bucket(packed_tokens(input_mask) if tokens is None else int(tokens), B, S)
+
+    def _graphed(self, key: tuple, args, run, train: bool, grad_scale: float = 1.0, what: str = "micro-step"):
+        """``run(*args)`` -- eager for the first ``graph_warmup`` calls of ``key``, then captured once and replayed with
+        ``args`` copied into the graph's static inputs.  Returns the program's output (the graph's own tensor when
+        replayed: valid until the next replay).
+
+        ``train``: the program draws dropout and writes gradients.  The capture runs it as ``run(*static,
+        seed=engine._seed_base)`` after advancing the device step counter, so that every replay draws fresh masks; the
+        fp8 weight copies are refreshed before every call, and ``grad_scale``, a launch constant, is part of the capture.
+        Otherwise (an evaluation) the step counter does not move."""
+        ent = self._graphs.setdefault(key, {"calls": 0})
+        ent["calls"] += 1
+        eng = self.engine
+        if train and "graph" in ent and ent["grad_scale"] != float(grad_scale):
+            # the loss scale is a launch constant: a GradScaler update invalidates the capture (rare); drop it
+            # (and its private memory pool) and capture again right away
+            for k in ("graph", "static", "out"):
+                ent.pop(k)
+        if "graph" not in ent:
+            if ent["calls"] <= self.graph_warmup or (eng.fp8 and not eng._fp8_calibrated):
+                return run(*args)
+            if train and self._seed_step is None:
+                self._seed_step = torch.zeros(1, dtype=torch.int64, device=self.arena.device)
+                ops.extension().set_seed_step(self._seed_step)
+            static = [None if t is None else t.clone() for t in args]
+            if train:
+                eng.prepare_step()
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            n0 = K.KERNEL_LAUNCHES
+            pool = next((e["graph"].pool() for e in self._graphs.values() if "graph" in e), None)
+            # replays never overlap: all captures share one memory pool; thread_local: a data-loader thread that pins
+            # or allocates memory while we capture must not abort the capture
+            extra = {}
+            if train and eng.wgrad_side:      # capture on a high-priority stream: the dgrad chain wins SMs over the wgrads
+                if self._cap_stream is None:
+                    self._cap_stream = torch.cuda.Stream(device=self.arena.device, priority=-1)
+                extra["stream"] = self._cap_stream
+            try:
+                with torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local", **extra):
+                    if train:
+                        self._seed_step.add_(1)
+                        out = run(*static, seed=eng._seed_base)
+                    else:                     # no dropout, and training's step counter must not move
+                        out = run(*static)
+            except Exception as e:            # e.g. an allocator / stream condition this build of torch cannot capture
+                warnings.warn(f"CUDA-graph capture of the {what} failed ({type(e).__name__}: {e}); "
+                              "continuing with the eager kernel program")
+                K.KERNEL_LAUNCHES = n0
+                self.use_graphs = False
+                torch.cuda.synchronize()      # nothing of the captured program ran: the accumulated gradients are intact
+                return run(*args)
+            ent.update(graph=graph, static=static, out=out, launches=K.KERNEL_LAUNCHES - n0, grad_scale=float(grad_scale))
+            K.KERNEL_LAUNCHES = n0            # the capture itself ran nothing
+        for dst, src in zip(ent["static"], args):
+            if dst is not None:
+                dst.copy_(src, non_blocking=True)
+        if train:
+            eng.prepare_step()
+        ent["graph"].replay()
+        K._count(ent["launches"])
+        return ent["out"]
+
+    def _eval_graphs_ok(self) -> bool:
+        return self.use_graphs and not _use_sdpa() and self.arena.device.type == "cuda"
+
+    def _keeping_fp8_table(self, fn):
+        """``fn()`` with the fp8 scaling table restored afterwards (the weight copies are refreshed first, as the next
+        micro-step would): an evaluation must not move the training's delayed scaling."""
+        eng = self.engine
+        table = None
+        if eng.fp8:
+            eng.prepare_step()
+            table = eng.meta.table.clone()
+        try:
+            return fn()
+        finally:
+            if table is not None:
+                eng.meta.table.copy_(table)
+
+
+class FusedPretrainer(_GraphedProgram):
+    """Forward + backward of ``BertForPreTraining`` + criterion as one kernel program.
+
+    ``forward_backward`` returns the (unscaled) loss of the micro-batch as a device scalar and leaves the
+    gradients -- multiplied by ``grad_scale`` (= loss_scale / accumulation_steps) -- accumulated in the arena.
+    """
+
+    def __init__(self, model):
+        super().__init__(model)
+        cfg = model.config
+        self.V, self.H = cfg.vocab_size, cfg.hidden_size
+        self.has_nsp = model.cls.has_nsp and model.bert.pooler is not None
+        self.max_pred = int(getattr(cfg, "max_predictions_per_seq", 0)) or None
+        self._loss = None
+        self.grad_push = False                # set by the runtime around the last micro-step (PeerComm.begin_push)
+        self._cls_idx = None                  # row indices of the [CLS] tokens (NSP head)
+        self._cls_S = 0
+        self._eval_cls: Dict[tuple, torch.Tensor] = {}   # [CLS] row indices of the evaluation batch shapes
+
+    def _max_pred(self, labels: torch.Tensor) -> int:
+        # capacity of masked positions per sequence; fixed per run so shapes stay static
+        if self.max_pred is None:
+            # no --max_predictions_per_seq: the capacity is the sequence length (any batch fits; the static-shape head
+            # then costs S rows per sequence, so runners should always pass the flag -- data/dataset.py validates
+            # pre-masked shards against it)
+            self.max_pred = (labels.size(1) + 7) // 8 * 8
+        return self.max_pred
 
     @torch.no_grad()
     def forward_backward(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
@@ -791,55 +885,8 @@ class FusedPretrainer:
                segment_ids is not None, tuple(str(t.dtype) for t in args if t is not None),
                bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)), self.engine.fp8,
                bool(self.grad_push), bool(self.engine.wgrad_side), K.deterministic(), bucket)
-        ent = self._graphs.setdefault(key, {"calls": 0})
-        ent["calls"] += 1
-        eng = self.engine
-        if "graph" in ent and ent["grad_scale"] != float(grad_scale):
-            # the loss scale is a launch constant: a GradScaler update invalidates the capture (rare); drop it
-            # (and its private memory pool) and capture again right away
-            for k in ("graph", "static", "loss"):
-                ent.pop(k)
-        if "graph" not in ent:
-            if ent["calls"] <= self.graph_warmup or (eng.fp8 and not eng._fp8_calibrated):
-                return self._program(*args, grad_scale, bucket=bucket)
-            if self._seed_step is None:
-                self._seed_step = torch.zeros(1, dtype=torch.int64, device=self.arena.device)
-                ops.extension().set_seed_step(self._seed_step)
-            self._max_pred(masked_lm_labels.to(torch.int32))
-            static = [None if t is None else t.clone() for t in args]
-            eng.prepare_step()
-            torch.cuda.synchronize()
-            graph = torch.cuda.CUDAGraph()
-            n0 = K.KERNEL_LAUNCHES
-            pool = next((e["graph"].pool() for e in self._graphs.values() if "graph" in e), None)
-            # replays never overlap: all captures share one memory pool; thread_local: a data-loader thread that pins
-            # or allocates memory while we capture must not abort the capture
-            extra = {}
-            if eng.wgrad_side:                # capture on a high-priority stream: the dgrad chain wins SMs over the wgrads
-                if self._cap_stream is None:
-                    self._cap_stream = torch.cuda.Stream(device=self.arena.device, priority=-1)
-                extra["stream"] = self._cap_stream
-            try:
-                with torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local", **extra):
-                    self._seed_step.add_(1)
-                    loss = self._program(*static, grad_scale, seed=eng._seed_base, bucket=bucket)
-            except Exception as e:            # e.g. an allocator / stream condition this build of torch cannot capture
-                import warnings
-                warnings.warn(f"CUDA-graph capture of the micro-step failed ({type(e).__name__}: {e}); "
-                              "continuing with the eager kernel program")
-                K.KERNEL_LAUNCHES = n0
-                self.use_graphs = False
-                torch.cuda.synchronize()      # nothing of the captured program ran: the accumulated gradients are intact
-                return self._program(*args, grad_scale, bucket=bucket)
-            ent.update(graph=graph, static=static, loss=loss, launches=K.KERNEL_LAUNCHES - n0, grad_scale=float(grad_scale))
-            K.KERNEL_LAUNCHES = n0            # the capture itself ran nothing
-        for dst, src in zip(ent["static"], args):
-            if dst is not None:
-                dst.copy_(src, non_blocking=True)
-        eng.prepare_step()
-        ent["graph"].replay()
-        K._count(ent["launches"])
-        return ent["loss"]
+        return self._graphed(key, args, lambda *a, seed=None: self._program(*a, grad_scale, seed=seed, bucket=bucket),
+                             train=True, grad_scale=grad_scale)
 
     @torch.no_grad()
     def _program(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
@@ -941,59 +988,20 @@ class FusedPretrainer:
         training graphs' memory pool."""
         if acc.dtype != torch.float64 or acc.numel() != 6:
             raise ValueError("evaluate: acc must be an fp64 tensor of 6 elements")
-        eng = self.engine
         bucket = self._bucket(input_mask, tokens, kfac=False)
         args = (input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels)
-        table = None
-        if eng.fp8:
-            eng.prepare_step()
-            table = eng.meta.table.clone()
-        try:
-            part = self._eval_replay(args, bucket)
-            acc += part
-        finally:
-            if table is not None:
-                eng.meta.table.copy_(table)
+        acc += self._keeping_fp8_table(lambda: self._eval_replay(args, bucket))
         return acc
 
     def _eval_replay(self, args, bucket) -> torch.Tensor:
         """The evaluation program of ``args``, eager or as a replayed CUDA graph; returns its fp64 [6] sums."""
-        eng = self.engine
-        if not (self.use_graphs and not _use_sdpa() and self.arena.device.type == "cuda"):
-            return self._eval_program(*args, bucket=bucket)
+        run = lambda *a: self._eval_program(*a, bucket=bucket)      # noqa: E731
+        if not self._eval_graphs_ok():
+            return run(*args)
         input_ids, segment_ids, _, _, next_sentence_labels = args
         key = ("eval", tuple(input_ids.shape), next_sentence_labels is not None, segment_ids is not None,
-               tuple(str(t.dtype) for t in args if t is not None), eng.fp8, K.deterministic(), bucket)
-        ent = self._graphs.setdefault(key, {"calls": 0})
-        ent["calls"] += 1
-        if "graph" not in ent:
-            if ent["calls"] <= self.graph_warmup or (eng.fp8 and not eng._fp8_calibrated):
-                return self._eval_program(*args, bucket=bucket)
-            self._max_pred(args[3].to(torch.int32))
-            static = [None if t is None else t.clone() for t in args]
-            torch.cuda.synchronize()
-            graph = torch.cuda.CUDAGraph()
-            n0 = K.KERNEL_LAUNCHES
-            pool = next((e["graph"].pool() for e in self._graphs.values() if "graph" in e), None)
-            try:
-                # no seed-step increment in here: the program has no dropout, and training's counter must not move
-                with torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local"):
-                    part = self._eval_program(*static, bucket=bucket)
-            except Exception as e:
-                warnings.warn(f"CUDA-graph capture of the evaluation failed ({type(e).__name__}: {e}); "
-                              "continuing with the eager kernel program")
-                K.KERNEL_LAUNCHES = n0
-                self.use_graphs = False
-                torch.cuda.synchronize()
-                return self._eval_program(*args, bucket=bucket)
-            ent.update(graph=graph, static=static, part=part, launches=K.KERNEL_LAUNCHES - n0)
-            K.KERNEL_LAUNCHES = n0
-        for dst, src in zip(ent["static"], args):
-            if dst is not None:
-                dst.copy_(src, non_blocking=True)
-        ent["graph"].replay()
-        K._count(ent["launches"])
-        return ent["part"]
+               tuple(str(t.dtype) for t in args if t is not None), self.engine.fp8, K.deterministic(), bucket)
+        return self._graphed(key, args, run, train=False, what="evaluation")
 
     @torch.no_grad()
     def _eval_program(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
@@ -1030,3 +1038,113 @@ class FusedPretrainer:
             K.nsp_eval(pooled, A.shadow("cls.seq_relationship.weight"), self.model.cls.seq_relationship.bias,
                        next_sentence_labels.long().view(-1).contiguous(), part[3:6])
         return part
+
+
+class FusedClassifier(_GraphedProgram):
+    """Fine-tuning and evaluation of ``BertForSequenceClassification`` (GLUE) as one kernel program each.
+
+    Training (``train_step``): [device packing] -> encoder forward -> gather of the [CLS] rows -> pooler GEMM with the
+    bias + tanh epilogue -> ``cls_head`` (dropout, classifier, cross-entropy and their backward in one launch) -> pooler
+    wgrad / bias / dgrad -> the [CLS]-row gradient into a zero sequence gradient -> encoder backward.  The classifier
+    dropout draws from stream :data:`CLS_STREAM` with the encoder's seed, so a replayed graph draws new masks as the
+    device step counter advances.  Evaluation (``predict``): the forward without dropout, ending in fp32 logits.  Both
+    follow the pre-training policy for buckets and graphs: one graph per (batch shape, bucket, mode), all in one pool.
+    Rows whose label is -1 are inert: a batch filled up to the static batch size with such rows (one unmasked token,
+    label -1) replays the same graph and its mean loss is over the real rows only."""
+
+    def __init__(self, model):
+        super().__init__(model)
+        if model.bert.pooler is None:
+            raise ValueError("FusedClassifier: the model has no pooler (config.next_sentence is false)")
+        if model.num_labels not in K.CLS_CLASSES:
+            raise ValueError(f"FusedClassifier: {model.num_labels} labels; the classifier kernel is built for "
+                             f"{K.CLS_CLASSES} classes")
+        self.H = model.config.hidden_size
+        self._cls: Dict[tuple, torch.Tensor] = {}    # [CLS] row indices of the padded batch shapes (never replaced:
+                                                     # captured graphs keep reading them)
+
+    def _cls_rows(self, pk: Optional[Packing], B: int, S: int, device) -> torch.Tensor:
+        if pk is not None:
+            return pk.cls_rows
+        idx = self._cls.get((B, S))
+        if idx is None:
+            idx = self._cls[(B, S)] = torch.arange(B, device=device, dtype=torch.int32) * S
+        return idx
+
+    def _pooled(self, seq, cls_idx):
+        eng, A = self.engine, self.arena
+        cls_tok = K.gather_rows(seq, cls_idx)                                                  # [B, H] bf16
+        pooled = K.gemm(cls_tok, A.shadow(eng.prefix + "pooler.dense_act.weight"), epi=K.EPI_BIAS_TANH,
+                        bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
+        return cls_tok, pooled
+
+    @torch.no_grad()
+    def train_step(self, input_ids, segment_ids, input_mask, labels, grad_scale: float = 1.0,
+                   tokens: Optional[int] = None) -> torch.Tensor:
+        """Forward, loss and backward of one batch: returns the mean cross-entropy over the rows whose label is not -1
+        (a device scalar) and accumulates the gradients, times ``grad_scale``, in the arena.  Unpadded
+        (``BertModel.unpad``) the batch is packed into the token bucket of ``tokens`` (its unmasked token count, a host
+        int; read back from the device when omitted)."""
+        bucket = self._bucket(input_mask, tokens)
+        run = lambda *a, seed=None: self._program(*a, grad_scale, seed=seed, bucket=bucket)   # noqa: E731
+        args = (input_ids, segment_ids, input_mask, labels)
+        if not self._graph_ok():
+            return run(*args)
+        key = ("cls", tuple(input_ids.shape), self.model.training, segment_ids is not None,
+               tuple(str(t.dtype) for t in args if t is not None),
+               bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)), self.engine.fp8,
+               bool(self.engine.wgrad_side), K.deterministic(), bucket)
+        return self._graphed(key, args, run, train=True, grad_scale=grad_scale)
+
+    @torch.no_grad()
+    def _program(self, input_ids, segment_ids, input_mask, labels, grad_scale: float = 1.0, seed: Optional[int] = None,
+                 bucket=None) -> torch.Tensor:
+        eng, A, H = self.engine, self.arena, self.H
+        B, S = input_ids.shape
+        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
+        M = pk.T if pk is not None else B * S
+        seq, sv = eng.forward(input_ids, segment_ids, input_mask, training=True, seed=seed, dropout=self.model.training,
+                              pack=pk)
+        cls_idx = self._cls_rows(pk, B, S, seq.device)
+        cls_tok, pooled = self._pooled(seq, cls_idx)
+        loss = torch.zeros(1, dtype=torch.float32, device=seq.device)
+        pool, clf = self.model.bert.pooler.dense_act, self.model.classifier
+        d_z = K.cls_head_(pooled, A.shadow("classifier.weight"), clf.bias, labels.long().view(-1).contiguous(),
+                          grad_scale, loss, clf.weight.grad, clf.bias.grad, p_drop=sv.p_hidden, seed=sv.seed,
+                          stream=CLS_STREAM)
+        pw = A.shadow(eng.prefix + "pooler.dense_act.weight")
+        K.wgrad_accumulate(d_z, cls_tok, pool.weight.grad)
+        K.colsum_accumulate(d_z, pool.bias.grad)
+        d_cls = K.gemm(d_z, pw, layout=K.NN)
+        # the sequence gradient is zero but at the (distinct) [CLS] rows: a scatter is the whole add, in every mode
+        d_seq = torch.zeros(M, H, dtype=torch.bfloat16, device=seq.device)
+        K.scatter_rows(d_cls, cls_idx, d_seq)
+        eng.backward(sv, d_seq)
+        return loss.squeeze(0)
+
+    @torch.no_grad()
+    def predict(self, input_ids, segment_ids, input_mask, tokens: Optional[int] = None) -> torch.Tensor:
+        """fp32 logits [B, C] of one batch: the forward without dropout.  Leaves the training state as it was: no
+        activation saved, no gradient written, the seed counters, ``model.training`` and the fp8 scaling table unmoved.
+        Graphs under keys of their own, in the training graphs' pool."""
+        bucket = self._bucket(input_mask, tokens, kfac=False)
+        args = (input_ids, segment_ids, input_mask)
+        run = lambda *a: self._eval_program(*a, bucket=bucket)                                 # noqa: E731
+
+        def go():
+            if not self._eval_graphs_ok():
+                return run(*args)
+            key = ("cls-eval", tuple(input_ids.shape), segment_ids is not None,
+                   tuple(str(t.dtype) for t in args if t is not None), self.engine.fp8, K.deterministic(), bucket)
+            return self._graphed(key, args, run, train=False, what="evaluation").clone()
+        return self._keeping_fp8_table(go)
+
+    @torch.no_grad()
+    def _eval_program(self, input_ids, segment_ids, input_mask, bucket=None) -> torch.Tensor:
+        eng, A = self.engine, self.arena
+        B, S = input_ids.shape
+        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
+        # an explicit seed: the engine's call counter, which numbers the training dropout seeds, stays where it is
+        seq, _ = eng.forward(input_ids, segment_ids, input_mask, training=False, seed=0, dropout=False, pack=pk)
+        _, pooled = self._pooled(seq, self._cls_rows(pk, B, S, seq.device))
+        return K.cls_logits(pooled, A.shadow("classifier.weight"), self.model.classifier.bias)

@@ -683,6 +683,7 @@ class BertForSequenceClassification(BertPreTrainedModel):
         self.bert = BertModel(config)
         self.dropout = nn.Dropout(config.hidden_dropout_prob)
         self.classifier = nn.Linear(config.hidden_size, num_labels)
+        self._classifier = None
         self.apply(self.init_bert_weights)
 
     def forward(self, input_ids, token_type_ids=None, attention_mask=None, labels=None):
@@ -691,6 +692,55 @@ class BertForSequenceClassification(BertPreTrainedModel):
         if labels is not None:
             return F.cross_entropy(logits.view(-1, self.num_labels).float(), labels.view(-1))
         return logits
+
+    def classifier_engine(self):
+        """The fused sm_90a training / evaluation program of this model (:class:`~.fused.FusedClassifier`), or
+        ``None`` where it cannot run: ``_can_fuse`` fails for ``input_ids``, the model has no pooler, or the label count
+        is not one the classifier kernel is built for (2 or 3)."""
+        from ..ops.api import CLS_CLASSES
+        if self.bert.pooler is None or self.num_labels not in CLS_CLASSES:
+            return None
+        if self._classifier is None:
+            from .fused import FusedClassifier
+            self._classifier = FusedClassifier(self)
+        return self._classifier
+
+    def _fused(self, input_ids):
+        return self.classifier_engine() if self.bert._can_fuse(input_ids) else None
+
+    def train_step(self, input_ids, token_type_ids, attention_mask, labels, grad_scale: float = 1.0,
+                   tokens: Optional[int] = None) -> torch.Tensor:
+        """Forward, loss and backward of one batch: returns the mean cross-entropy over the rows whose label is not -1
+        and accumulates the gradients (times ``grad_scale``) into ``.grad``.  Through the fused program
+        (:meth:`~.fused.FusedClassifier.train_step`, dropout as ``self.training`` says) where it runs, else the plain
+        PyTorch forward and backward (autocast is the caller's).  ``tokens``: the unmasked token count of the batch
+        (a host int) for the unpadded program's bucket."""
+        eng = self._fused(input_ids)
+        if eng is not None:
+            return eng.train_step(input_ids, token_type_ids, attention_mask, labels, grad_scale, tokens=tokens)
+        logits = self(input_ids.long(), None if token_type_ids is None else token_type_ids.long(), attention_mask.long())
+        loss = F.cross_entropy(logits.view(-1, self.num_labels).float(), labels.long().view(-1), ignore_index=-1)
+        if not bool((labels >= 0).any()):
+            loss = logits.sum() * 0.0          # every row ignored: loss 0 and zero gradients, not NaN
+        (loss * grad_scale).backward()
+        return loss.detach()
+
+    @torch.no_grad()
+    def predict(self, input_ids, token_type_ids, attention_mask, tokens: Optional[int] = None) -> torch.Tensor:
+        """fp32 logits [B, num_labels] without dropout.  Through the fused program
+        (:meth:`~.fused.FusedClassifier.predict`) where it runs, else the plain PyTorch forward in eval mode (autocast
+        is the caller's); ``self.training`` is left as it was."""
+        eng = self._fused(input_ids)
+        if eng is not None:
+            return eng.predict(input_ids, token_type_ids, attention_mask, tokens=tokens)
+        was = self.training
+        self.eval()
+        try:
+            logits = self(input_ids.long(), None if token_type_ids is None else token_type_ids.long(),
+                          attention_mask.long())
+        finally:
+            self.train(was)
+        return logits.float()
 
 
 class BertForMultipleChoice(BertPreTrainedModel):

@@ -380,6 +380,41 @@ def nsp_head_(pooled: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, labels:
     return dz
 
 
+CLS_CLASSES = (2, 3)    # the instantiated class counts of cls_head (the GLUE classification tasks)
+
+
+def _check_classes(w: torch.Tensor) -> None:
+    if w.dim() != 2 or w.size(0) not in CLS_CLASSES:
+        raise ValueError(f"cls_head: {w.size(0) if w.dim() == 2 else '?'} classes; the kernel is built for "
+                         f"C in {CLS_CLASSES}")
+
+
+def cls_head_(pooled: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, labels: torch.Tensor, grad_scale: float,
+              loss_out: torch.Tensor, dw: torch.Tensor, db: torch.Tensor, p_drop: float = 0.0, seed: int = 0,
+              stream: int = 0) -> torch.Tensor:
+    """Sequence-classification head after the pooler in one launch: dropout ``p_drop`` on the pooled bf16 [B, H]
+    (Philox ``(seed, stream)``, element ``b * H + i``), logits = dropped @ ``w``^T + ``bias`` (``w`` bf16 [C, H], C = 2
+    or 3; fp32 ``bias``), and mean cross-entropy over the rows whose int64 label lies in [0, C).  ``loss_out`` += the
+    mean, ``dw`` / ``db`` (fp32) accumulate the classifier gradients (atomics, or per-row partials added in order in
+    deterministic mode); returns dz = d loss / d (pooler pre-activation) [B, H] bf16 (dropout and tanh' folded in).
+    With no valid row the loss and every gradient are zero."""
+    _check_classes(w)
+    dz = torch.empty_like(pooled)
+    det = deterministic()
+    extension().cls_head(pooled, w, bias, labels, grad_scale, seed, stream, p_drop, loss_out, dz, dw, db, det)
+    _count(4 if det else 1)
+    return dz
+
+
+def cls_logits(pooled: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """Evaluation form of :func:`cls_head_`: fp32 logits [B, C] of the pooled bf16 [B, H], without dropout."""
+    _check_classes(w)
+    out = torch.empty(pooled.size(0), w.size(0), dtype=torch.float32, device=pooled.device)
+    extension().cls_logits(pooled, w, bias, out)
+    _count()
+    return out
+
+
 def softmax_ce_(logits: torch.Tensor, targets: torch.Tensor, count: torch.Tensor, grad_scale: float,
                 loss_out: torch.Tensor) -> None:
     """In place: logits <- d loss / d logits (scaled); loss_out += mean CE over valid targets."""

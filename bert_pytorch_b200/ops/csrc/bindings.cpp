@@ -609,6 +609,47 @@ void nsp_head(Tensor pooled, Tensor w, Tensor bias, Tensor labels, double grad_s
                  cur_stream(), deterministic ? f32_workspace(dw, B * (3 + 2 * H)).data_ptr<float>() : nullptr);
 }
 
+inline void check_cls(const Tensor& pooled, const Tensor& w, const Tensor& bias, const char* name) {
+  check_bf16(pooled, "pooled"); check_bf16(w, "w");
+  TORCH_CHECK(pooled.dim() == 2 && pooled.is_contiguous() && pooled.size(1) % 8 == 0, name,
+              ": pooled must be a contiguous [B, H] with H % 8 == 0");
+  TORCH_CHECK(w.dim() == 2 && w.is_contiguous() && (w.size(0) == 2 || w.size(0) == 3) && w.size(1) == pooled.size(1), name,
+              ": w must be a contiguous [C, H] with C = 2 or 3");
+  TORCH_CHECK(bias.is_cuda() && bias.device() == pooled.device() && bias.scalar_type() == at::kFloat && bias.is_contiguous() &&
+              bias.numel() == w.size(0), name, ": bias must be a contiguous fp32 CUDA tensor [C]");
+}
+
+void cls_head(Tensor pooled, Tensor w, Tensor bias, Tensor labels, double grad_scale, int64_t seed, int64_t stream_id,
+              double p_drop, Tensor loss_out, Tensor dz, Tensor dw, Tensor db, bool deterministic) {
+  check_cls(pooled, w, bias, "cls_head");
+  check_bf16(dz, "dz");
+  const int64_t B = pooled.size(0), H = pooled.size(1), C = w.size(0);
+  TORCH_CHECK(dz.is_contiguous() && dz.sizes() == pooled.sizes(), "cls_head: dz must be a contiguous tensor of pooled's shape");
+  TORCH_CHECK(labels.is_cuda() && labels.device() == pooled.device() && labels.scalar_type() == at::kLong &&
+              labels.is_contiguous() && labels.numel() == B, "cls_head: labels must be a contiguous int64 CUDA tensor [B]");
+  TORCH_CHECK(dw.is_cuda() && dw.scalar_type() == at::kFloat && dw.is_contiguous() && dw.numel() == C * H &&
+              db.is_cuda() && db.scalar_type() == at::kFloat && db.is_contiguous() && db.numel() == C &&
+              loss_out.is_cuda() && loss_out.scalar_type() == at::kFloat && loss_out.numel() >= 1,
+              "cls_head: fp32 gradient buffers dw [C, H], db [C] and loss");
+  TORCH_CHECK(p_drop >= 0.0 && p_drop < 1.0, "cls_head: p_drop must lie in [0, 1)");
+  c10::cuda::CUDAGuard guard(pooled.device());
+  b200::cls_head(pooled.data_ptr(), w.data_ptr(), bias.data_ptr<float>(),
+                 reinterpret_cast<const long long*>(labels.data_ptr<int64_t>()), (int)B, (int)H, (int)C, (float)grad_scale,
+                 mk_seed(seed), (unsigned)stream_id, (float)p_drop, loss_out.data_ptr<float>(), dz.data_ptr(),
+                 dw.data_ptr<float>(), db.data_ptr<float>(), cur_stream(),
+                 deterministic ? f32_workspace(dw, B * (1 + C + C * H)).data_ptr<float>() : nullptr);
+}
+
+void cls_logits(Tensor pooled, Tensor w, Tensor bias, Tensor logits) {
+  check_cls(pooled, w, bias, "cls_logits");
+  const int64_t B = pooled.size(0), C = w.size(0);
+  TORCH_CHECK(logits.is_cuda() && logits.device() == pooled.device() && logits.scalar_type() == at::kFloat &&
+              logits.is_contiguous() && logits.numel() == B * C, "cls_logits: logits must be a contiguous fp32 [B, C]");
+  c10::cuda::CUDAGuard guard(pooled.device());
+  b200::cls_logits(pooled.data_ptr(), w.data_ptr(), bias.data_ptr<float>(), (int)B, (int)pooled.size(1), (int)C,
+                   logits.data_ptr<float>(), cur_stream());
+}
+
 // evaluation metrics: rows fp32 [R, 3] ({loss, correct, valid} per row), sums fp32 [3] += their column sums (in order)
 inline void check_eval_out(const Tensor& rows, const Tensor& sums, int64_t R, const Tensor& like, const char* name) {
   TORCH_CHECK(rows.is_cuda() && rows.device() == like.device() && rows.scalar_type() == at::kFloat && rows.is_contiguous() &&
@@ -729,6 +770,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("scatter_rows", &scatter_rows);
   m.def("softmax_ce", &softmax_ce);
   m.def("nsp_head", &nsp_head);
+  m.def("cls_head", &cls_head);
+  m.def("cls_logits", &cls_logits);
   m.def("mlm_eval", &mlm_eval);
   m.def("nsp_eval", &nsp_eval);
   m.def("mt_l2norm", &mt_l2norm);

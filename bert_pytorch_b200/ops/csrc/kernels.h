@@ -133,6 +133,15 @@ void nsp_head(const void* pooled_bf16, const void* w_bf16, const float* bias, co
               float grad_scale, float* loss_out, void* dz_bf16, float* dw, float* db, cudaStream_t st,
               float* rows_ws = nullptr);   // rows_ws [B * (3 + 2 H)]: deterministic mode
 
+// loss.cu: sequence-classification head (dropout + [B,H] x [H,C] classifier + CE + backward) in one launch, C = 2 or 3;
+// pooled / w / dz bf16 with H % 8 == 0, labels int64 (outside [0, C): ignored)
+void cls_head(const void* pooled_bf16, const void* w_bf16, const float* bias, const long long* labels, int B, int H, int C,
+              float grad_scale, Seed seed, unsigned int stream, float p_drop, float* loss_out, void* dz_bf16, float* dw,
+              float* db, cudaStream_t st, float* rows_ws = nullptr);   // rows_ws [B * (1 + C + C H)]: deterministic mode
+// evaluation form: fp32 logits [B, C], no dropout
+void cls_logits(const void* pooled_bf16, const void* w_bf16, const float* bias, int B, int H, int C, float* logits,
+                cudaStream_t st);
+
 // loss.cu: evaluation metrics, forward only.  rows [R, 3] receives {loss, correct, valid} of every row ({0, 0, 0} for an
 // ignored one); sums [3] += the column sums of rows, added by ordered_sum (no atomics, the same bits in every mode).
 // mlm_eval: bf16 logits [R, V] (V % 8 == 0, row stride ld), targets int32 (< 0: ignored).  nsp_eval: pooled bf16 [B, H],

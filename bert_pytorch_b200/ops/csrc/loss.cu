@@ -229,6 +229,219 @@ void nsp_head(const void* pooled, const void* w, const float* bias, const long l
 }
 
 // ------------------------------------------------------------------------------------------------
+// Sequence-classification head (GLUE fine-tuning), everything after the pooler GEMM in ONE launch: dropout on the
+// pooled row (keep decisions from Philox stream `stream` at element index b * H + i, rescale 1 / (1 - p)), the
+// [B, H] x [H, C] classifier, its cross-entropy (mean over the rows whose label lies in [0, C); any other label is
+// ignored), and the backward: db[C], dW[C, H] and  dz = (dlogits . W) * keep / (1 - p) * (1 - pooled^2).  One block per
+// sequence; C (2 or 3, the GLUE classification tasks) is a template parameter so that the logits stay in registers.
+// ROWS (deterministic mode): sequence b stores its loss term, db and dW contributions to loss_out[b], db[C b + c] and
+// dw[C H b + c H + i] (zeros when it contributes nothing) for ordered_sum, instead of atomics.
+// ------------------------------------------------------------------------------------------------
+constexpr int CLS_THREADS = 128;
+
+// 8 consecutive pooled values of group g (elements 8 g .. 8 g + 7 of the row) and their dropout multipliers
+__device__ __forceinline__ void cls_load8(const __nv_bfloat16* __restrict__ x, int g, float (&xv)[8]) {
+  const uint4 u = reinterpret_cast<const uint4*>(x)[g];
+  const uint32_t wd[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    const float2 p = unpack_bf16(wd[t]);
+    xv[2 * t] = p.x; xv[2 * t + 1] = p.y;
+  }
+}
+
+__device__ __forceinline__ void cls_keep8(unsigned long long seed, unsigned stream, unsigned thresh16, float keep_scale,
+                                          unsigned long long e8, float (&mul)[8]) {
+  if (thresh16 == 0u) {
+#pragma unroll
+    for (int t = 0; t < 8; ++t) mul[t] = 1.f;
+    return;
+  }
+  const Keep8 k = dropout_keep8(seed, stream, e8, thresh16);
+#pragma unroll
+  for (int t = 0; t < 8; ++t) mul[t] = k[t] ? keep_scale : 0.f;
+}
+
+// the C partial sums of every thread added over the block in a fixed order; every thread gets the totals
+template <int C>
+__device__ __forceinline__ void cls_block_sum(float (&a)[C], float* sm) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    const float v = warp_sum(a[c]);
+    if (lane == 0) sm[warp * C + c] = v;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    float r = 0.f;
+    for (int k = 0; k < CLS_THREADS / 32; ++k) r += sm[k * C + c];
+    a[c] = r;
+  }
+  __syncthreads();
+}
+
+// logits of row x (H % 8 == 0) after the dropout multipliers of its elements (all 1 without dropout)
+template <int C>
+__device__ __forceinline__ void cls_logits_row(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ w,
+                                               const float* __restrict__ bias, int H, unsigned long long seed,
+                                               unsigned stream, unsigned thresh16, float keep_scale,
+                                               unsigned long long e8_row, float (&l)[C], float* sm) {
+#pragma unroll
+  for (int c = 0; c < C; ++c) l[c] = 0.f;
+  for (int g = threadIdx.x; g < (H >> 3); g += CLS_THREADS) {
+    float xv[8], mul[8];
+    cls_load8(x, g, xv);
+    cls_keep8(seed, stream, thresh16, keep_scale, e8_row + (unsigned long long)g, mul);
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      float wv[8];
+      cls_load8(w + (size_t)c * H, g, wv);
+#pragma unroll
+      for (int t = 0; t < 8; ++t) l[c] += xv[t] * mul[t] * wv[t];
+    }
+  }
+  cls_block_sum<C>(l, sm);
+#pragma unroll
+  for (int c = 0; c < C; ++c) l[c] += bias[c];
+}
+
+template <int C, bool ROWS>
+__global__ void __launch_bounds__(CLS_THREADS)
+cls_head_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w, const float* __restrict__ bias,
+                const long long* __restrict__ labels, int B, int H, float grad_scale, Seed seed, unsigned stream,
+                unsigned thresh16, float keep_scale, float* __restrict__ loss_out, __nv_bfloat16* __restrict__ dz,
+                float* __restrict__ dw, float* __restrict__ db) {
+  __shared__ float sm[(CLS_THREADS / 32) * C];
+  const int b = blockIdx.x;
+  int n_valid = 0;
+  for (int i = 0; i < B; ++i) n_valid += (labels[i] >= 0 && labels[i] < C) ? 1 : 0;   // B is small: no second launch
+  const long long y = labels[b];
+  const bool live = y >= 0 && y < C;                 // then n_valid >= 1
+  const __nv_bfloat16* x = pooled + (size_t)b * H;
+  const unsigned long long sd = seed.value();
+  const unsigned long long e8_row = (unsigned long long)b * (unsigned long long)(H >> 3);
+  float l[C];
+  cls_logits_row<C>(x, w, bias, H, sd, stream, thresh16, keep_scale, e8_row, l, sm);
+  float d[C];
+#pragma unroll
+  for (int c = 0; c < C; ++c) d[c] = 0.f;
+  if constexpr (ROWS) {
+    loss_out += b; db += C * b; dw += (size_t)C * H * b;
+  }
+  float term = 0.f;
+  if (live) {
+    float m = l[0], ly = l[0];
+#pragma unroll
+    for (int c = 1; c < C; ++c) {
+      m = fmaxf(m, l[c]);
+      if (c == y) ly = l[c];
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int c = 0; c < C; ++c) s += expf(l[c] - m);
+    const float lse = m + logf(s);
+    const float inv = 1.f / (float)n_valid;
+    term = (lse - ly) * inv;
+#pragma unroll
+    for (int c = 0; c < C; ++c) d[c] = (expf(l[c] - lse) - (c == y ? 1.f : 0.f)) * inv * grad_scale;
+  }
+  if (threadIdx.x == 0) {
+    if constexpr (ROWS) {
+      *loss_out = term;
+#pragma unroll
+      for (int c = 0; c < C; ++c) db[c] = d[c];
+    } else if (live) {
+      atomicAdd(loss_out, term);
+#pragma unroll
+      for (int c = 0; c < C; ++c) atomicAdd(db + c, d[c]);
+    }
+  }
+  for (int g = threadIdx.x; g < (H >> 3); g += CLS_THREADS) {
+    float xv[8], mul[8], dx[8];
+    cls_load8(x, g, xv);
+    cls_keep8(sd, stream, thresh16, keep_scale, e8_row + (unsigned long long)g, mul);
+#pragma unroll
+    for (int t = 0; t < 8; ++t) dx[t] = 0.f;
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      float wv[8];
+      cls_load8(w + (size_t)c * H, g, wv);
+#pragma unroll
+      for (int t = 0; t < 8; ++t) dx[t] += d[c] * wv[t];
+    }
+    float o[8];
+#pragma unroll
+    for (int t = 0; t < 8; ++t) o[t] = dx[t] * mul[t] * (1.f - xv[t] * xv[t]);
+    reinterpret_cast<uint4*>(dz + (size_t)b * H)[g] =
+        make_uint4(pack_bf16(o[0], o[1]), pack_bf16(o[2], o[3]), pack_bf16(o[4], o[5]), pack_bf16(o[6], o[7]));
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      float* dwc = dw + (size_t)c * H + 8 * g;
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const float v = d[c] * xv[t] * mul[t];
+        if constexpr (ROWS) dwc[t] = live ? v : 0.f;
+        else if (live) atomicAdd(dwc + t, v);
+      }
+    }
+  }
+}
+
+// evaluation form: fp32 logits [B, C] of the pooled rows, no dropout, the training kernel's dot-product order
+template <int C>
+__global__ void __launch_bounds__(CLS_THREADS)
+cls_logits_kernel(const __nv_bfloat16* __restrict__ pooled, const __nv_bfloat16* __restrict__ w,
+                  const float* __restrict__ bias, int H, float* __restrict__ logits) {
+  __shared__ float sm[(CLS_THREADS / 32) * C];
+  float l[C];
+  cls_logits_row<C>(pooled + (size_t)blockIdx.x * H, w, bias, H, 0ull, 0u, 0u, 1.f, 0ull, l, sm);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int c = 0; c < C; ++c) logits[(size_t)blockIdx.x * C + c] = l[c];
+  }
+}
+
+template <int C>
+static void cls_head_launch(const void* pooled, const void* w, const float* bias, const long long* labels, int B, int H,
+                            float grad_scale, Seed seed, unsigned stream, float p_drop, float* loss_out, void* dz,
+                            float* dw, float* db, cudaStream_t st, float* rows_ws) {
+  const unsigned thresh = p_drop > 0.f ? (unsigned)(p_drop * 65536.f + 0.5f) : 0u;
+  const float scale = p_drop > 0.f ? 65536.f / (65536.f - (float)thresh) : 1.f;
+  const auto* x = (const __nv_bfloat16*)pooled;
+  const auto* wb = (const __nv_bfloat16*)w;
+  if (rows_ws == nullptr) {
+    cls_head_kernel<C, false><<<B, CLS_THREADS, 0, st>>>(x, wb, bias, labels, B, H, grad_scale, seed, stream, thresh,
+                                                         scale, loss_out, (__nv_bfloat16*)dz, dw, db);
+    return;
+  }
+  float* loss_rows = rows_ws;                 // [B], then db [B, C], then dW [B, C, H]
+  float* db_rows = rows_ws + B;
+  float* dw_rows = rows_ws + (size_t)(1 + C) * B;
+  cls_head_kernel<C, true><<<B, CLS_THREADS, 0, st>>>(x, wb, bias, labels, B, H, grad_scale, seed, stream, thresh, scale,
+                                                      loss_rows, (__nv_bfloat16*)dz, dw_rows, db_rows);
+  ordered_sum(loss_rows, B, 1, nullptr, 1, loss_out, st);
+  ordered_sum(db_rows, B, C, nullptr, 1, db, st);
+  ordered_sum(dw_rows, B, C * H, nullptr, 1, dw, st);
+}
+
+void cls_head(const void* pooled, const void* w, const float* bias, const long long* labels, int B, int H, int C,
+              float grad_scale, Seed seed, unsigned stream, float p_drop, float* loss_out, void* dz, float* dw, float* db,
+              cudaStream_t st, float* rows_ws) {
+  if (B <= 0) return;
+  if (C == 2) cls_head_launch<2>(pooled, w, bias, labels, B, H, grad_scale, seed, stream, p_drop, loss_out, dz, dw, db, st, rows_ws);
+  else if (C == 3) cls_head_launch<3>(pooled, w, bias, labels, B, H, grad_scale, seed, stream, p_drop, loss_out, dz, dw, db, st, rows_ws);
+}
+
+void cls_logits(const void* pooled, const void* w, const float* bias, int B, int H, int C, float* logits, cudaStream_t st) {
+  if (B <= 0) return;
+  const auto* x = (const __nv_bfloat16*)pooled;
+  const auto* wb = (const __nv_bfloat16*)w;
+  if (C == 2) cls_logits_kernel<2><<<B, CLS_THREADS, 0, st>>>(x, wb, bias, H, logits);
+  else if (C == 3) cls_logits_kernel<3><<<B, CLS_THREADS, 0, st>>>(x, wb, bias, H, logits);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Evaluation metrics (forward only; the inputs are only read).  Every row r writes rows[r] = {loss, correct, valid}:
 // the cross-entropy of its target, whether the argmax is the target, and 1 -- or {0, 0, 0} for an ignored row.  The
 // rows are then added by ordered_sum in a fixed order: no atomics, so the sums are the same bits in every mode.
