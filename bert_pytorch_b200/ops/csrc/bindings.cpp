@@ -196,14 +196,25 @@ bool gemm_timeline(c10::optional<Tensor> buf) {
 inline void check_ln_width(int64_t H) {
   TORCH_CHECK(H > 0 && H % 8 == 0 && H <= 2048, "LayerNorm: hidden size ", H, " is not a multiple of 8 in [8, 2048]");
 }
+// fp32 CUDA vector of n elements; `vec16`: read with 16-byte loads (gamma / beta), so its start must be 16-byte aligned
+inline void check_f32_vec(const Tensor& t, int64_t n, const char* name, bool vec16) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous(), name, " must be a contiguous CUDA fp32 tensor");
+  TORCH_CHECK(t.numel() == n, name, " has ", t.numel(), " elements, expected ", n);
+  TORCH_CHECK(!vec16 || reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, name, " must be 16-byte aligned");
+}
+inline void check_opt_f32_vec(const c10::optional<Tensor>& t, int64_t n, const char* name) {
+  if (t.has_value() && t->defined()) check_f32_vec(*t, n, name, false);
+}
 
 void layer_norm_fwd(Tensor x,Tensor gamma, Tensor beta, Tensor y, c10::optional<Tensor> mean,
                     c10::optional<Tensor> rstd, double eps, c10::optional<Tensor> q8, c10::optional<Tensor> meta8,
                     bool e5m2) {
   check_ln_width(x.size(-1));
   check_bf16(x, "x"); check_bf16(y, "y");
-  TORCH_CHECK(x.is_contiguous() && y.is_contiguous(), "x/y must be contiguous");
+  TORCH_CHECK(x.is_contiguous() && y.is_contiguous() && y.numel() == x.numel(), "x/y must be contiguous and of one size");
   const int H = (int)x.size(-1), M = (int)(x.numel() / H);
+  check_f32_vec(gamma, H, "gamma", true); check_f32_vec(beta, H, "beta", true);
+  check_opt_f32_vec(mean, M, "mean"); check_opt_f32_vec(rstd, M, "rstd");
   c10::cuda::CUDAGuard guard(x.device());
   b200::layer_norm_fwd(x.data_ptr(), gamma.data_ptr<float>(), beta.data_ptr<float>(), y.data_ptr(), opt_f32(mean),
                        opt_f32(rstd), M, H, (float)eps, mk_fp8(q8, meta8, e5m2, x.numel()), cur_stream());
@@ -218,11 +229,20 @@ void layer_norm_bwd(Tensor dy, Tensor x, Tensor mean, Tensor rstd, Tensor gamma,
                     bool deterministic) {
   check_ln_width(x.size(-1));
   check_bf16(dy, "dy"); check_bf16(x, "x"); check_bf16(dx, "dx");
+  TORCH_CHECK(x.is_contiguous() && dy.is_contiguous() && dx.is_contiguous() && dy.numel() == x.numel() &&
+              dx.numel() == x.numel(), "dy/x/dx must be contiguous and of one size");
   const int H = (int)x.size(-1), M = (int)(x.numel() / H);
+  check_f32_vec(mean, M, "mean", false); check_f32_vec(rstd, M, "rstd", false);
+  check_f32_vec(gamma, H, "gamma", true);
+  check_opt_f32_vec(dgamma, H, "dgamma"); check_opt_f32_vec(dbeta, H, "dbeta"); check_opt_f32_vec(dbias, H, "dbias");
   TORCH_CHECK(workspace.numel() >= b200::ln_bwd_workspace_floats(M, H), "LN workspace too small");
   c10::cuda::CUDAGuard guard(x.device());
   void* dxd_p = nullptr;
-  if (dxd.has_value() && dxd->defined()) { check_bf16(*dxd, "dxd"); dxd_p = dxd->data_ptr(); }
+  if (dxd.has_value() && dxd->defined()) {
+    check_bf16(*dxd, "dxd");
+    TORCH_CHECK(dxd->is_contiguous() && dxd->numel() == x.numel(), "dxd must be contiguous and of the size of x");
+    dxd_p = dxd->data_ptr();
+  }
   const uint8_t* km = nullptr;
   if (keep_mask.has_value() && keep_mask->defined()) {   // keep bits written by the producing GEMM (GemmCall::mask_out)
     TORCH_CHECK(keep_mask->is_cuda() && keep_mask->scalar_type() == at::kByte && keep_mask->is_contiguous() &&
@@ -259,9 +279,12 @@ void colsum(Tensor x, Tensor out, bool deterministic) {
   check_bf16(x, "x");
   TORCH_CHECK(x.dim() == 2 && out.scalar_type() == at::kFloat && out.numel() == x.size(1), "colsum shapes");
   c10::cuda::CUDAGuard guard(x.device());
+  TORCH_CHECK(out.is_cuda() && out.is_contiguous(), "colsum: out must be a contiguous CUDA tensor");
   const int M = (int)x.size(0), N = (int)x.size(1);
+  // both kernels read 8 columns with one 16-byte load: unit column stride (check_bf16), N and the row stride in 8s
+  TORCH_CHECK(N % 8 == 0 && x.stride(0) % 8 == 0, "colsum: N and the row stride must be multiples of 8");
+  if (M == 0 || N == 0) return;
   if (deterministic) {
-    TORCH_CHECK(N % 8 == 0 && x.stride(0) % 8 == 0, "deterministic colsum: N and the row stride must be multiples of 8");
     Tensor ws = f32_workspace(out, b200::colsum_det_workspace_floats(M, N));
     b200::colsum_bf16_det(x.data_ptr(), M, N, (int)x.stride(0), out.data_ptr<float>(), ws.data_ptr<float>(), cur_stream());
     return;
@@ -293,15 +316,28 @@ void embedding_fwd(Tensor ids, c10::optional<Tensor> seg, Tensor word, Tensor po
                    double p_drop, int64_t seed, int64_t stream_id, c10::optional<Tensor> pos_ids) {
   TORCH_CHECK(ids.scalar_type() == at::kInt && ids.is_contiguous(), "ids must be contiguous int32");
   check_bf16(word, "word"); check_bf16(pos, "pos"); check_bf16(e_out, "e_out"); check_bf16(y, "y");
+  TORCH_CHECK(word.dim() == 2 && pos.dim() == 2 && word.is_contiguous() && pos.is_contiguous(),
+              "word / position tables must be contiguous [rows, H]");
   const int H = (int)word.size(1), M = (int)ids.numel();
+  check_ln_width(H);
+  TORCH_CHECK(pos.size(1) == H, "position table width ", pos.size(1), " != ", H);
+  TORCH_CHECK(S > 0, "embedding_fwd: S must be positive");
+  TORCH_CHECK(e_out.is_contiguous() && y.is_contiguous() && e_out.numel() == (int64_t)M * H && y.numel() == (int64_t)M * H,
+              "e_out / y must be contiguous [M, H]");
+  check_f32_vec(gamma, H, "gamma", true); check_f32_vec(beta, H, "beta", true);
+  check_f32_vec(mean, M, "mean", false); check_f32_vec(rstd, M, "rstd", false);
   c10::cuda::CUDAGuard guard(ids.device());
   const int* seg_p = nullptr;
   const void* type_p = nullptr;
   if (type.has_value() && type->defined()) {
-    TORCH_CHECK(seg.has_value() && seg->scalar_type() == at::kInt, "segment ids must be int32");
+    TORCH_CHECK(seg.has_value() && seg->defined() && seg->scalar_type() == at::kInt && seg->is_contiguous() &&
+                seg->numel() == M, "segment ids must be a contiguous int32 tensor like ids");
+    check_bf16(*type, "type");
+    TORCH_CHECK(type->dim() == 2 && type->is_contiguous() && type->size(1) == H, "token-type table must be contiguous [rows, H]");
     seg_p = seg->data_ptr<int>();
     type_p = type->data_ptr();
   }
+  if (M == 0) return;
   b200::embedding_fwd(ids.data_ptr<int>(), seg_p, word.data_ptr(), pos.data_ptr(), type_p, gamma.data_ptr<float>(),
                       beta.data_ptr<float>(), e_out.data_ptr(), y.data_ptr(), mean.data_ptr<float>(),
                       rstd.data_ptr<float>(), M, (int)S, H, (float)eps, mk_seed(seed), (unsigned)stream_id,
@@ -312,10 +348,22 @@ void embedding_bwd_scatter(Tensor de, Tensor ids, c10::optional<Tensor> seg, Ten
                            c10::optional<Tensor> gtype, int64_t S, c10::optional<Tensor> pos_ids, bool deterministic) {
   check_bf16(de, "de");
   const int H = (int)de.size(-1), M = (int)ids.numel();
+  check_ln_width(H);
+  TORCH_CHECK(ids.scalar_type() == at::kInt && ids.is_contiguous(), "ids must be contiguous int32");
+  TORCH_CHECK(de.is_contiguous() && de.numel() == (int64_t)M * H, "de must be contiguous [M, H]");
+  TORCH_CHECK(S > 0, "embedding backward: S must be positive");
+  auto check_table = [&](const Tensor& t, const char* name) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.is_contiguous() && t.dim() == 2 && t.size(1) == H &&
+                reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, name, " must be a contiguous 16-byte aligned fp32 [rows, H]");
+  };
+  check_table(gword, "gword"); check_table(gpos, "gpos");
+  if (gtype.has_value() && gtype->defined()) check_table(*gtype, "gtype");
+  if (seg.has_value() && seg->defined())
+    TORCH_CHECK(seg->scalar_type() == at::kInt && seg->is_contiguous() && seg->numel() == M,
+                "segment ids must be a contiguous int32 tensor like ids");
+  if (M == 0) return;
   c10::cuda::CUDAGuard guard(de.device());
   if (deterministic) {
-    TORCH_CHECK(H % 8 == 0 && de.is_contiguous(), "deterministic embedding backward: contiguous de with H % 8 == 0");
-    TORCH_CHECK(S > 0, "deterministic embedding backward: S must be positive");
     const int chunk = std::min(M, b200::embedding_det_chunk_rows());   // rows sorted at a time
     int64_t rows = std::max(gword.size(0), gpos.size(0));
     if (gtype.has_value() && gtype->defined()) rows = std::max(rows, gtype->size(0));

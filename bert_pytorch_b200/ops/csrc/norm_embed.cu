@@ -177,7 +177,10 @@ ln_fwd_row_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__
     for (int c = 0; c < CHUNKS; ++c)
 #pragma unroll
       for (int t = 0; t < 8; ++t) s += v[c][t];
-    const float mean = warp_sum(s) * (1.0f / (float)H);
+    // a true division: a row of equal values then has its own value as mean and a variance of exactly 0 (the sum is
+    // exact, but sum * (1/H) can land one ulp off for H not a power of two, which rstd ~ 1/sqrt(eps) turns into
+    // an error of order 0.1 * gamma)
+    const float mean = warp_sum(s) / (float)H;
     float q = 0.f;
 #pragma unroll
     for (int c = 0; c < CHUNKS; ++c)
@@ -602,7 +605,7 @@ embed_fwd_kernel(const int* __restrict__ ids, const int* __restrict__ seg, const
 }
 
 // Embedding backward scatter: de [M,H] (bf16) is added into the fp32 gradient tables (position row: pos_ids[row] when
-// given, else row % S).
+// given, else row % S; token-type row seg[row], or 0 without segment ids).
 __global__ void __launch_bounds__(256)
 embed_bwd_scatter_kernel(const __nv_bfloat16* __restrict__ de, const int* __restrict__ ids,
                          const int* __restrict__ seg, float* __restrict__ gword, float* __restrict__ gpos,
@@ -622,7 +625,7 @@ embed_bwd_scatter_kernel(const __nv_bfloat16* __restrict__ de, const int* __rest
     }
     float* dst[3] = {gword + (size_t)ids[row] * H + col,
                      gpos ? gpos + (size_t)(pos_ids ? pos_ids[row] : row % S) * H + col : nullptr,
-                     gtype ? gtype + (size_t)seg[row] * H + col : nullptr};
+                     gtype ? gtype + (size_t)(seg ? seg[row] : 0) * H + col : nullptr};
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       if (dst[k] == nullptr) continue;
@@ -1018,6 +1021,7 @@ static inline int ln_grid(int M) {
 
 void layer_norm_fwd(const void* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int M,
                     int H, float eps, Fp8Out f8, cudaStream_t st) {
+  if (M == 0) return;                    // no rows: a zero-sized grid is a launch error
   decltype(&ln_fwd_row_kernel<1, false, false>) k;
   if (f8.q == nullptr && H % 256 == 0 && H <= 1024)      // the encoder LNs of the bf16 path
     k = H == 256 ? ln_fwd_row_kernel<1, false, false> : H == 512 ? ln_fwd_row_kernel<2, false, false>
@@ -1049,6 +1053,7 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
                     void* dxd, float* dgamma, float* dbeta, float* dbias, float* workspace, int M, int H,
                     Seed seed, unsigned int drop_stream, unsigned int in_stream, float p_drop, Fp8Out f8,
                     cudaStream_t st, const uint8_t* keep_mask, bool deterministic) {
+  if (M == 0) return;                    // nothing to add to the column sums either
   unsigned int th; float sc;
   drop_params(p_drop, th, sc);
   decltype(&ln_bwd3_kernel<1, 8, false, false>) k;
@@ -1135,6 +1140,7 @@ void dgelu_bwd(const void* dy, const void* x, void* dx, float* dbias, int M, int
 void embedding_fwd(const int* ids, const int* seg, const void* word, const void* pos, const void* type,
                    const float* gamma, const float* beta, void* e_out, void* y, float* mean, float* rstd, int M, int S,
                    int H, float eps, Seed seed, unsigned int stream, float p_drop, cudaStream_t st, const int* pos_ids) {
+  if (M == 0) return;
   unsigned int th; float sc;
   drop_params(p_drop, th, sc);
   if (pos_ids != nullptr)
@@ -1149,6 +1155,7 @@ void embedding_fwd(const int* ids, const int* seg, const void* word, const void*
 
 void embedding_bwd_scatter(const void* de, const int* ids, const int* seg, float* gword, float* gpos, float* gtype,
                            int M, int S, int H, int type_rows, cudaStream_t st, const int* pos_ids) {
+  if (M == 0) return;
   const size_t work = (size_t)M * (H / 8);
   int grid = (int)((work + 255) / 256);
   if (grid > num_sms() * 16) grid = num_sms() * 16;
