@@ -37,6 +37,7 @@ the rows past the real tokens are [PAD] tokens in dummy sequences of their own, 
 """
 from __future__ import annotations
 
+import gc
 import math
 import os
 import warnings
@@ -69,10 +70,6 @@ def _as_tuple(x):
     return x if isinstance(x, tuple) else (x,)
 
 
-def _use_sdpa() -> bool:
-    return os.environ.get("B200_ATTN", "native") == "sdpa"
-
-
 @dataclass
 class _LayerSaved:
     x: torch.Tensor = None
@@ -90,7 +87,6 @@ class _LayerSaved:
     mask2: torch.Tensor = None      # GEMM epilogues, read back by the LayerNorm backward kernels
     mean2: torch.Tensor = None
     rstd2: torch.Tensor = None
-    sdpa: tuple = None
     x_op: torch.Tensor = None      # operands of the four weight-gradient GEMMs (bf16 tensors or their fp8 copies)
     ctx_op: torch.Tensor = None
     x1_op: torch.Tensor = None
@@ -189,8 +185,7 @@ class FusedEncoderEngine:
             raise NotImplementedError("the fused engine implements the erf-GELU FFN only")
         if self.H % 64 != 0 or (self.H // self.heads) != 64:
             # the attention kernel is specialised for head_dim 64 (every shipped config)
-            if not _use_sdpa():
-                raise NotImplementedError("fused attention needs head_dim == 64 (set B200_ATTN=sdpa otherwise)")
+            raise NotImplementedError("fused attention needs head_dim == 64")
         ref = getattr(bert, "_arena_ref", None)
         arena = ref() if ref is not None else None
         if arena is None:
@@ -406,8 +401,6 @@ class FusedEncoderEngine:
 
         ckpt = training and bool(getattr(self.bert.encoder, "_checkpoint_activations", False))
         seg_len = int(math.ceil(math.sqrt(self.L))) if ckpt else 0
-        if ckpt and _use_sdpa():
-            raise NotImplementedError("B200_ATTN=sdpa (library bring-up path) cannot replay its dropout under --checkpoint_activations")
         for l in range(self.L):
             if ckpt and l % seg_len == 0:
                 sv.boundaries[l] = x             # --checkpoint_activations: keep segment inputs only (K27)
@@ -424,17 +417,11 @@ class FusedEncoderEngine:
         """One post-LN transformer layer (reference: src/modeling.py:482-499) as 9 kernel launches.  ``x``: [B*S, H],
         or [T, H] packed rows with ``pk``."""
         A, H, M = self.arena, self.H, x.size(0)
-        training = save or pa > 0 or ph > 0
         pre = f"encoder.layer.{l}."
         ls = _LayerSaved() if save else None
         qkv, x_op = self._lin(l, "x", "wqkv", x, self._qkv(l, A.flat_shadow, "weight"), xq=xq, epi=K.EPI_BIAS,
                               bias=self._qkv(l, A.flat_shadow, "bias"))
-        if _use_sdpa():
-            ctx, lse, sd = self._sdpa_fwd(qkv, seqlens, B, S, pa, training)
-            ctx_q = None
-            if save:
-                ls.sdpa = sd
-        elif pk is not None:
+        if pk is not None:
             ctx, lse = K.attention_fwd(qkv, None, self.heads, p_drop=pa, seed=seed, stream=_stream(l, SITE_ATTN_PROB),
                                        cu_seqlens=pk.cu_seqlens, S=S)
             ctx_q = None
@@ -568,9 +555,7 @@ class FusedEncoderEngine:
                               self.g(pre + "attention.output.dense.weight"), dyq=q[0] if q else None)
         # ---- attention core
         dqkv_q = None
-        if ls.sdpa is not None:
-            d_qkv = self._sdpa_bwd(ls.sdpa, d_ctx, sv.B, sv.S)
-        elif sv.pk is not None:
+        if sv.pk is not None:
             d_qkv = K.attention_bwd(ls.qkv, None, ls.ctx, d_ctx, ls.lse, self.heads, p_drop=pa, seed=seed,
                                     stream=_stream(l, SITE_ATTN_PROB), cu_seqlens=sv.pk.cu_seqlens, S=sv.S)
         else:
@@ -589,39 +574,15 @@ class FusedEncoderEngine:
         self._wgrad_layer_done()
         return d
 
-    # -- library attention (bring-up / bisecting aid: B200_ATTN=sdpa) ---------------------------------
-    def _sdpa_fwd(self, qkv, seqlens, B, S, p, training):
-        H, h = self.H, self.heads
-        d = H // h
-        t = qkv.view(B, S, 3, h, d)
-        q, k, v = (t[:, :, i].transpose(1, 2) for i in range(3))
-        # the kernels' rule: an all-zero mask row (length 0) attends to every key
-        n = torch.where(seqlens > 0, seqlens, S)
-        mask = (torch.arange(S, device=qkv.device)[None, :] < n[:, None])[:, None, None, :]
-        if training:
-            with torch.enable_grad():
-                q, k, v = (z.detach().requires_grad_(True) for z in (q, k, v))
-                o = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=p)
-            return o.detach().transpose(1, 2).reshape(B * S, H), None, (q, k, v, o)
-        o = F.scaled_dot_product_attention(q, k, v, attn_mask=mask)
-        return o.transpose(1, 2).reshape(B * S, H), None, None
-
-    def _sdpa_bwd(self, sd, d_ctx, B, S):
-        q, k, v, o = sd
-        H, h = self.H, self.heads
-        go = d_ctx.view(B, S, h, H // h).transpose(1, 2)
-        dq, dk, dv = torch.autograd.grad(o, (q, k, v), go)
-        return torch.stack([dq.transpose(1, 2), dk.transpose(1, 2), dv.transpose(1, 2)], dim=2).reshape(B * S, 3 * H)
-
     # -- autograd bridge for models with ordinary torch heads (finetuning, inference) ------------------
     def _packing(self, attention_mask) -> Optional[Packing]:
         """The packing of this batch when ``BertModel.unpad`` is set and the unpadded path can serve the engine's
-        configuration (fp8 operands and the library attention run padded), else None."""
+        configuration (fp8 operands run padded), else None."""
         if not getattr(self.bert, "unpad", False):
             return None
-        if self.fp8 or _use_sdpa():
+        if self.fp8:
             if not getattr(self, "_unpad_warned", False):
-                warnings.warn("BertModel.unpad: fp8 operands and B200_ATTN=sdpa have no unpadded path; running padded")
+                warnings.warn("BertModel.unpad: fp8 operands have no unpadded path; running padded")
                 self._unpad_warned = True
             return None
         return pack_rows(attention_mask)
@@ -709,16 +670,16 @@ def head_linear(linear: torch.nn.Linear, x: torch.Tensor) -> torch.Tensor:
     64 outputs, at least 128 rows -- smaller problems are launch bound either way), else the module itself."""
     H = x.size(-1)
     rows = x.numel() // max(H, 1)
-    if (x.is_cuda and ops.available() and H % 8 == 0 and linear.out_features <= 64 and rows >= 128
-            and os.environ.get("B200_HEAD_GEMM", "1") != "0"):
+    if x.is_cuda and ops.available() and H % 8 == 0 and linear.out_features <= 64 and rows >= 128:
         return _HeadLinearFn.apply(x, linear.weight, linear.bias)
     return linear(x)
 
 
 class _GraphedProgram:
-    """What the fused training programs share: the token bucket of an unpadded batch, and the policy that runs a
-    kernel program eagerly for its first ``graph_warmup`` calls per input signature, then captures it once and replays
-    it as one CUDA graph, every capture in one memory pool."""
+    """What the fused programs share: the token bucket of an unpadded batch, the steps every program starts with
+    (packing, encoder forward, [CLS] rows, pooler), the CUDA-graph key, and the policy that runs a kernel program
+    eagerly for its first ``graph_warmup`` calls per input signature, then captures it once and replays it as one CUDA
+    graph, every capture in one memory pool."""
 
     def __init__(self, model):
         self.model = model
@@ -731,25 +692,25 @@ class _GraphedProgram:
         self._graphs: Dict[tuple, dict] = {}
         self._seed_step: Optional[torch.Tensor] = None
         self._cap_stream = None               # high-priority capture stream (wgrad side-stream mode)
+        self._cls: Dict[tuple, torch.Tensor] = {}    # [CLS] row indices of the padded batch shapes
 
     def _graph_ok(self) -> bool:
         kf = getattr(self.model.bert, "_kfac", None)
-        if not self.use_graphs or _use_sdpa() or (kf is not None and getattr(kf, "capture", True)):
-            return False                      # tapped micro-steps keep Python-side state; the library attention path owns its RNG
+        if not self.use_graphs or (kf is not None and getattr(kf, "capture", True)):
+            return False                      # tapped micro-steps keep Python-side state
         return self.arena.device.type == "cuda"
 
     def _bucket(self, input_mask, tokens: Optional[int], kfac: bool = True):
-        """(T_cap, D) of this micro-step when it runs unpadded (``BertModel.unpad``), else None.  fp8 operands and the
-        library attention have no unpadded path (warned once), and K-FAC micro-steps that feed the factors run padded
-        so that their statistics are the padded ones (``kfac=False``: an evaluation, which feeds nothing).  Without
-        ``tokens`` the count is read back from the device (one host sync)."""
+        """(T_cap, D) of this micro-step when it runs unpadded (``BertModel.unpad``), else None.  fp8 operands have no
+        unpadded path (warned once), and K-FAC micro-steps that feed the factors run padded so that their statistics
+        are the padded ones (``kfac=False``: an evaluation, which feeds nothing).  Without ``tokens`` the count is read
+        back from the device (one host sync)."""
         if not getattr(self.model.bert, "unpad", False):
             return None
-        eng = self.engine
-        if eng.fp8 or _use_sdpa():
+        if self.engine.fp8:
             if not getattr(self, "_unpad_warned", False):
-                warnings.warn("BertModel.unpad: fp8 operands and B200_ATTN=sdpa have no unpadded pre-training path or "
-                              "classification program; running padded")
+                warnings.warn("BertModel.unpad: fp8 operands have no unpadded pre-training path or classification "
+                              "program; running padded")
                 self._unpad_warned = True
             return None
         kf = getattr(self.model.bert, "_kfac", None)
@@ -757,6 +718,48 @@ class _GraphedProgram:
             return None
         B, S = input_mask.shape
         return token_bucket(packed_tokens(input_mask) if tokens is None else int(tokens), B, S)
+
+    def _encode(self, input_ids, segment_ids, input_mask, bucket, train: bool, seed: Optional[int] = None):
+        """The start of every program: the device packing of the batch into ``bucket`` (padded without one), then the
+        encoder forward -- ``train``: saving activations, with dropout as ``model.training`` says; otherwise without
+        dropout.  Returns (sequence output, saved-or-None, packing-or-None, its row count M)."""
+        B, S = input_ids.shape
+        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
+        M = pk.T if pk is not None else B * S
+        # an evaluation passes an explicit seed: the engine's call counter, which numbers the training dropout seeds,
+        # stays where it is
+        seq, sv = self.engine.forward(input_ids, segment_ids, input_mask, training=train, seed=seed if train else 0,
+                                      dropout=train and self.model.training, pack=pk)
+        return seq, sv, pk, M
+
+    def _cls_rows(self, pk: Optional[Packing], B: int, S: int, device) -> torch.Tensor:
+        """Rows of the [CLS] tokens in the sequence output: the first packed row of every sequence, or b * S.  The
+        padded indices are one tensor per (B, S), never replaced or evicted: captured graphs keep reading them."""
+        if pk is not None:
+            return pk.cls_rows
+        idx = self._cls.get((B, S))
+        if idx is None:
+            idx = self._cls[(B, S)] = torch.arange(B, device=device, dtype=torch.int32) * S
+        return idx
+
+    def _pooled(self, seq, cls_idx):
+        """(the [CLS] rows [B, H] bf16, the pooler output): a gather, then a GEMM with the bias + tanh epilogue."""
+        eng, A = self.engine, self.arena
+        cls_tok = K.gather_rows(seq, cls_idx)
+        pooled = K.gemm(cls_tok, A.shadow(eng.prefix + "pooler.dense_act.weight"), epi=K.EPI_BIAS_TANH,
+                        bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
+        return cls_tok, pooled
+
+    def _graph_key(self, kind: str, args, bucket, train: bool, *extra) -> tuple:
+        """CUDA-graph key of one call: ``kind``, the batch shape, the dtype of every argument (None where absent), the
+        fp8 mode; for a training program its mode, activation checkpointing, the weight-gradient stream and ``extra``;
+        then the deterministic mode and, last, the token bucket."""
+        eng = self.engine
+        key = (kind, tuple(args[0].shape), tuple(None if t is None else t.dtype for t in args), eng.fp8)
+        if train:
+            key += (self.model.training, bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)),
+                    bool(eng.wgrad_side), *extra)
+        return key + (K.deterministic(), bucket)
 
     def _graphed(self, key: tuple, args, run, train: bool, grad_scale: float = 1.0, what: str = "micro-step"):
         """``run(*args)`` -- eager for the first ``graph_warmup`` calls of ``key``, then captured once and replayed with
@@ -795,6 +798,11 @@ class _GraphedProgram:
                 if self._cap_stream is None:
                     self._cap_stream = torch.cuda.Stream(device=self.arena.device, priority=-1)
                 extra["stream"] = self._cap_stream
+            # no cyclic garbage collection inside the capture: it could destroy the CUDA graphs and events of programs
+            # that are no longer referenced (a model and its engine form reference cycles), and a CUDA call of this
+            # thread that is not capturable invalidates the capture
+            gc_on = gc.isenabled()
+            gc.disable()
             try:
                 with torch.cuda.graph(graph, pool=pool, capture_error_mode="thread_local", **extra):
                     if train:
@@ -809,6 +817,9 @@ class _GraphedProgram:
                 self.use_graphs = False
                 torch.cuda.synchronize()      # nothing of the captured program ran: the accumulated gradients are intact
                 return run(*args)
+            finally:
+                if gc_on:
+                    gc.enable()
             ent.update(graph=graph, static=static, out=out, launches=K.KERNEL_LAUNCHES - n0, grad_scale=float(grad_scale))
             K.KERNEL_LAUNCHES = n0            # the capture itself ran nothing
         for dst, src in zip(ent["static"], args):
@@ -821,7 +832,7 @@ class _GraphedProgram:
         return ent["out"]
 
     def _eval_graphs_ok(self) -> bool:
-        return self.use_graphs and not _use_sdpa() and self.arena.device.type == "cuda"
+        return self.use_graphs and self.arena.device.type == "cuda"
 
     def _keeping_fp8_table(self, fn):
         """``fn()`` with the fp8 scaling table restored afterwards (the weight copies are refreshed first, as the next
@@ -853,9 +864,6 @@ class FusedPretrainer(_GraphedProgram):
         self.max_pred = int(getattr(cfg, "max_predictions_per_seq", 0)) or None
         self._loss = None
         self.grad_push = False                # set by the runtime around the last micro-step (PeerComm.begin_push)
-        self._cls_idx = None                  # row indices of the [CLS] tokens (NSP head)
-        self._cls_S = 0
-        self._eval_cls: Dict[tuple, torch.Tensor] = {}   # [CLS] row indices of the evaluation batch shapes
 
     def _max_pred(self, labels: torch.Tensor) -> int:
         # capacity of masked positions per sequence; fixed per run so shapes stay static
@@ -881,10 +889,7 @@ class FusedPretrainer(_GraphedProgram):
             return self._program(input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels, grad_scale,
                                  bucket=bucket)
         args = (input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels)
-        key = (tuple(input_ids.shape), self.model.training, next_sentence_labels is not None,
-               segment_ids is not None, tuple(str(t.dtype) for t in args if t is not None),
-               bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)), self.engine.fp8,
-               bool(self.grad_push), bool(self.engine.wgrad_side), K.deterministic(), bucket)
+        key = self._graph_key("train", args, bucket, True, bool(self.grad_push))
         return self._graphed(key, args, lambda *a, seed=None: self._program(*a, grad_scale, seed=seed, bucket=bucket),
                              train=True, grad_scale=grad_scale)
 
@@ -893,29 +898,20 @@ class FusedPretrainer(_GraphedProgram):
                  grad_scale: float = 1.0, seed: Optional[int] = None, bucket=None) -> torch.Tensor:
         """The kernel program of one micro-step; ``bucket`` = (T_cap, D) runs it on the packed tokens of the batch
         (T_cap rows: the real tokens, then a pad tail of inert [PAD] rows in D dummy sequences)."""
-        eng, A, H, V = self.engine, self.arena, self.H, self.V
+        eng, A, H = self.engine, self.arena, self.H
         B, S = input_ids.shape
-        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
-        M = pk.T if pk is not None else B * S
-        seq, sv = eng.forward(input_ids, segment_ids, input_mask, training=True, seed=seed, dropout=self.model.training,
-                              pack=pk)
+        seq, sv, pk, M = self._encode(input_ids, segment_ids, input_mask, bucket, train=True, seed=seed)
         labels = masked_lm_labels.to(torch.int32).contiguous()
         mp = self._max_pred(labels)
         idx, tgt, count = K.mlm_compact(labels, mp, row_map=pk.row_map if pk is not None else None)
         loss = torch.zeros(1, dtype=torch.float32, device=seq.device)
 
         # ---- MLM head forward (masked rows only)
-        rows = K.gather_rows(seq, idx)
-        t_pre = K.gemm(rows, A.shadow("cls.predictions.transform.dense_act.weight"), epi=K.EPI_BIAS,
-                       bias=A.shadow("cls.predictions.transform.dense_act.bias"))
-        t_act = K.gelu_fwd(t_pre)
-        t_ln, t_mean, t_rstd = K.layer_norm_fwd(t_act, A.view("cls.predictions.transform.LayerNorm.weight"),
-                                                A.view("cls.predictions.transform.LayerNorm.bias"))
-        emb_w = eng.w("embeddings.word_embeddings.weight")            # tied decoder weight [V, H]
-        logits = K.gemm(t_ln, emb_w, epi=K.EPI_BIAS, bias=A.shadow("cls.predictions.bias"))
+        logits, (rows, t_pre, t_act, t_ln, t_mean, t_rstd) = self._mlm_forward(seq, idx, save_stats=True)
         K.softmax_ce_(logits, tgt, count, grad_scale, loss)            # logits <- dlogits
 
         # ---- MLM head backward
+        emb_w = eng.w("embeddings.word_embeddings.weight")            # tied decoder weight [V, H]
         K.colsum_accumulate(logits, A.grad("cls.predictions.bias"))
         d_t_ln = K.gemm(logits, emb_w, layout=K.NN)
         K.wgrad_accumulate(logits, t_ln, eng.g("embeddings.word_embeddings.weight"))
@@ -933,16 +929,8 @@ class FusedPretrainer(_GraphedProgram):
         #      dgrad / wgrad GEMMs (M = B rows)
         if self.has_nsp and next_sentence_labels is not None:
             pool, nsp = self.model.bert.pooler.dense_act, self.model.cls.seq_relationship
-            pw = A.shadow(eng.prefix + "pooler.dense_act.weight")
-            if pk is not None:
-                cls_idx = pk.cls_rows
-            else:
-                if self._cls_idx is None or self._cls_idx.numel() != B or self._cls_S != S:
-                    self._cls_idx = (torch.arange(B, device=seq.device, dtype=torch.int32) * S).contiguous()
-                    self._cls_S = S
-                cls_idx = self._cls_idx
-            cls_tok = K.gather_rows(seq, cls_idx)                                              # [B, H] bf16
-            pooled = K.gemm(cls_tok, pw, epi=K.EPI_BIAS_TANH, bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
+            cls_idx = self._cls_rows(pk, B, S, seq.device)
+            cls_tok, pooled = self._pooled(seq, cls_idx)
             d_z = K.nsp_head_(pooled, A.shadow("cls.seq_relationship.weight"), nsp.bias, next_sentence_labels.long().view(-1),
                               grad_scale, loss, nsp.weight.grad, nsp.bias.grad)
             kf = getattr(self.model.bert, "_kfac", None)
@@ -958,7 +946,7 @@ class FusedPretrainer(_GraphedProgram):
                 kf.tap("cls.seq_relationship", pooled, d_lg)
             K.wgrad_accumulate(d_z, cls_tok, pool.weight.grad)
             K.colsum_accumulate(d_z, pool.bias.grad)
-            d_cls = K.gemm(d_z, pw, layout=K.NN)
+            d_cls = K.gemm(d_z, A.shadow(eng.prefix + "pooler.dense_act.weight"), layout=K.NN)
             if pk is not None and K.deterministic():
                 # torch's deterministic index_add_ sorts its indices; the rows are distinct, so gather, add and scatter
                 # back instead: the same bf16 add, on the engine's kernels
@@ -970,6 +958,21 @@ class FusedPretrainer(_GraphedProgram):
 
         eng.backward(sv, d_seq)
         return loss.squeeze(0) if loss.dim() else loss
+
+    def _mlm_forward(self, seq, idx, save_stats: bool):
+        """The MLM head on the masked rows ``idx`` of the sequence output: gather -> transform GEMM + bias -> GELU ->
+        LayerNorm (with its row statistics when ``save_stats``) -> tied decoder GEMM + bias.  Returns (logits [rows,
+        V], (rows, t_pre, t_act, t_ln, t_mean, t_rstd)), the intermediates the backward reads."""
+        A = self.arena
+        rows = K.gather_rows(seq, idx)
+        t_pre = K.gemm(rows, A.shadow("cls.predictions.transform.dense_act.weight"), epi=K.EPI_BIAS,
+                       bias=A.shadow("cls.predictions.transform.dense_act.bias"))
+        t_act = K.gelu_fwd(t_pre)
+        t_ln, t_mean, t_rstd = K.layer_norm_fwd(t_act, A.view("cls.predictions.transform.LayerNorm.weight"),
+                                                A.view("cls.predictions.transform.LayerNorm.bias"), save_stats=save_stats)
+        logits = K.gemm(t_ln, self.engine.w("embeddings.word_embeddings.weight"), epi=K.EPI_BIAS,
+                        bias=A.shadow("cls.predictions.bias"))
+        return logits, (rows, t_pre, t_act, t_ln, t_mean, t_rstd)
 
     # -- evaluation ------------------------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -998,44 +1001,25 @@ class FusedPretrainer(_GraphedProgram):
         run = lambda *a: self._eval_program(*a, bucket=bucket)      # noqa: E731
         if not self._eval_graphs_ok():
             return run(*args)
-        input_ids, segment_ids, _, _, next_sentence_labels = args
-        key = ("eval", tuple(input_ids.shape), next_sentence_labels is not None, segment_ids is not None,
-               tuple(str(t.dtype) for t in args if t is not None), self.engine.fp8, K.deterministic(), bucket)
-        return self._graphed(key, args, run, train=False, what="evaluation")
+        return self._graphed(self._graph_key("eval", args, bucket, False), args, run, train=False, what="evaluation")
 
     @torch.no_grad()
     def _eval_program(self, input_ids, segment_ids, input_mask, masked_lm_labels, next_sentence_labels,
                       bucket=None) -> torch.Tensor:
         """Encoder forward without dropout, the MLM head on the masked rows and the NSP head on the [CLS] rows, then the
         metric kernels.  Returns fp64 [6]: the MLM sums {loss, correct, count}, then the NSP sums."""
-        eng, A = self.engine, self.arena
         B, S = input_ids.shape
-        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
-        # an explicit seed: the engine's call counter, which numbers the training dropout seeds, stays where it is
-        seq, _ = eng.forward(input_ids, segment_ids, input_mask, training=False, seed=0, dropout=False, pack=pk)
+        seq, _, pk, _ = self._encode(input_ids, segment_ids, input_mask, bucket, train=False)
         labels = masked_lm_labels.to(torch.int32).contiguous()
         idx, tgt, _ = K.mlm_compact(labels, self._max_pred(labels), row_map=pk.row_map if pk is not None else None)
         part = torch.zeros(6, dtype=torch.float64, device=seq.device)
 
-        rows = K.gather_rows(seq, idx)
-        t_pre = K.gemm(rows, A.shadow("cls.predictions.transform.dense_act.weight"), epi=K.EPI_BIAS,
-                       bias=A.shadow("cls.predictions.transform.dense_act.bias"))
-        t_ln, _, _ = K.layer_norm_fwd(K.gelu_fwd(t_pre), A.view("cls.predictions.transform.LayerNorm.weight"),
-                                      A.view("cls.predictions.transform.LayerNorm.bias"), save_stats=False)
-        logits = K.gemm(t_ln, eng.w("embeddings.word_embeddings.weight"), epi=K.EPI_BIAS, bias=A.shadow("cls.predictions.bias"))
+        logits, _ = self._mlm_forward(seq, idx, save_stats=False)
         K.mlm_eval(logits, tgt, part[0:3])
 
         if self.has_nsp and next_sentence_labels is not None:
-            if pk is not None:
-                cls_idx = pk.cls_rows
-            else:
-                # a cache of its own: a captured training graph keeps reading the training batch's index tensor
-                cls_idx = self._eval_cls.get((B, S))
-                if cls_idx is None:
-                    cls_idx = self._eval_cls[(B, S)] = torch.arange(B, device=seq.device, dtype=torch.int32) * S
-            pooled = K.gemm(K.gather_rows(seq, cls_idx), A.shadow(eng.prefix + "pooler.dense_act.weight"),
-                            epi=K.EPI_BIAS_TANH, bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
-            K.nsp_eval(pooled, A.shadow("cls.seq_relationship.weight"), self.model.cls.seq_relationship.bias,
+            _, pooled = self._pooled(seq, self._cls_rows(pk, B, S, seq.device))
+            K.nsp_eval(pooled, self.arena.shadow("cls.seq_relationship.weight"), self.model.cls.seq_relationship.bias,
                        next_sentence_labels.long().view(-1).contiguous(), part[3:6])
         return part
 
@@ -1060,23 +1044,6 @@ class FusedClassifier(_GraphedProgram):
             raise ValueError(f"FusedClassifier: {model.num_labels} labels; the classifier kernel is built for "
                              f"{K.CLS_CLASSES} classes")
         self.H = model.config.hidden_size
-        self._cls: Dict[tuple, torch.Tensor] = {}    # [CLS] row indices of the padded batch shapes (never replaced:
-                                                     # captured graphs keep reading them)
-
-    def _cls_rows(self, pk: Optional[Packing], B: int, S: int, device) -> torch.Tensor:
-        if pk is not None:
-            return pk.cls_rows
-        idx = self._cls.get((B, S))
-        if idx is None:
-            idx = self._cls[(B, S)] = torch.arange(B, device=device, dtype=torch.int32) * S
-        return idx
-
-    def _pooled(self, seq, cls_idx):
-        eng, A = self.engine, self.arena
-        cls_tok = K.gather_rows(seq, cls_idx)                                                  # [B, H] bf16
-        pooled = K.gemm(cls_tok, A.shadow(eng.prefix + "pooler.dense_act.weight"), epi=K.EPI_BIAS_TANH,
-                        bias=A.shadow(eng.prefix + "pooler.dense_act.bias"))
-        return cls_tok, pooled
 
     @torch.no_grad()
     def train_step(self, input_ids, segment_ids, input_mask, labels, grad_scale: float = 1.0,
@@ -1090,21 +1057,14 @@ class FusedClassifier(_GraphedProgram):
         args = (input_ids, segment_ids, input_mask, labels)
         if not self._graph_ok():
             return run(*args)
-        key = ("cls", tuple(input_ids.shape), self.model.training, segment_ids is not None,
-               tuple(str(t.dtype) for t in args if t is not None),
-               bool(getattr(self.model.bert.encoder, "_checkpoint_activations", False)), self.engine.fp8,
-               bool(self.engine.wgrad_side), K.deterministic(), bucket)
-        return self._graphed(key, args, run, train=True, grad_scale=grad_scale)
+        return self._graphed(self._graph_key("cls", args, bucket, True), args, run, train=True, grad_scale=grad_scale)
 
     @torch.no_grad()
     def _program(self, input_ids, segment_ids, input_mask, labels, grad_scale: float = 1.0, seed: Optional[int] = None,
                  bucket=None) -> torch.Tensor:
         eng, A, H = self.engine, self.arena, self.H
         B, S = input_ids.shape
-        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
-        M = pk.T if pk is not None else B * S
-        seq, sv = eng.forward(input_ids, segment_ids, input_mask, training=True, seed=seed, dropout=self.model.training,
-                              pack=pk)
+        seq, sv, pk, M = self._encode(input_ids, segment_ids, input_mask, bucket, train=True, seed=seed)
         cls_idx = self._cls_rows(pk, B, S, seq.device)
         cls_tok, pooled = self._pooled(seq, cls_idx)
         loss = torch.zeros(1, dtype=torch.float32, device=seq.device)
@@ -1134,17 +1094,13 @@ class FusedClassifier(_GraphedProgram):
         def go():
             if not self._eval_graphs_ok():
                 return run(*args)
-            key = ("cls-eval", tuple(input_ids.shape), segment_ids is not None,
-                   tuple(str(t.dtype) for t in args if t is not None), self.engine.fp8, K.deterministic(), bucket)
+            key = self._graph_key("cls-eval", args, bucket, False)
             return self._graphed(key, args, run, train=False, what="evaluation").clone()
         return self._keeping_fp8_table(go)
 
     @torch.no_grad()
     def _eval_program(self, input_ids, segment_ids, input_mask, bucket=None) -> torch.Tensor:
-        eng, A = self.engine, self.arena
         B, S = input_ids.shape
-        pk = pack_device(input_mask, input_ids, segment_ids, *bucket) if bucket is not None else None
-        # an explicit seed: the engine's call counter, which numbers the training dropout seeds, stays where it is
-        seq, _ = eng.forward(input_ids, segment_ids, input_mask, training=False, seed=0, dropout=False, pack=pk)
+        seq, _, pk, _ = self._encode(input_ids, segment_ids, input_mask, bucket, train=False)
         _, pooled = self._pooled(seq, self._cls_rows(pk, B, S, seq.device))
-        return K.cls_logits(pooled, A.shadow("classifier.weight"), self.model.classifier.bias)
+        return K.cls_logits(pooled, self.arena.shadow("classifier.weight"), self.model.classifier.bias)

@@ -504,7 +504,7 @@ class BertModel(BertPreTrainedModel):
     positions as attention over the valid keys.  This is exact for every head that never reads masked positions --
     token classification with its masked loss, sequence classification, multiple choice and QA prediction -- but not
     for QA training, whose start / end cross-entropy normalises over all positions, masked ones included.
-    fp8 operands and ``B200_ATTN=sdpa`` have no unpadded path: they run padded (with a warning)."""
+    fp8 operands have no unpadded path: they run padded (with a warning)."""
 
     def __init__(self, config: BertConfig):
         super().__init__(config)
@@ -541,7 +541,7 @@ class BertModel(BertPreTrainedModel):
             return False
         H, h = cfg.hidden_size, cfg.num_attention_heads
         if H % 64 != 0 or H // h != 64:
-            return os.environ.get("B200_ATTN", "native") == "sdpa" and H % 8 == 0
+            return False
         if cfg.intermediate_size % 8 != 0 or H > 8 * 256:
             return False
         return True

@@ -135,7 +135,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   const int b = bh / p.h, head = bh % p.h;
   int seqlen, row0;
   if constexpr (VARLEN) {
-    pdl_wait();                                         // cu_seqlens may come from the previous kernel
     row0 = p.seqlens[b];
     seqlen = min(p.seqlens[b + 1] - row0, p.S);
     if (qb * QT >= seqlen) return;                      // CTA uniform, before any mbarrier or TMA work
@@ -156,8 +155,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     fence_barrier_init();
   }
   __syncthreads();
-  if constexpr (!VARLEN) pdl_wait();
-  pdl_trigger_small();
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(&bars[0], 8192);
     tma_load_2d(sQ, &tmap_q, &bars[0], head * HD, row0 + qb * QT);
@@ -557,7 +554,7 @@ static void launch_fwd(const void* qkv, const AttnArgs& a, long long rows, cudaS
     B200_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured = smem;
   }
-  launch_pdl(attn_fwd_kernel<VARLEN>, dim3((S + QT - 1) / QT, a.B * a.h), dim3(128), (size_t)smem, st, tq, tkv, a);
+  attn_fwd_kernel<VARLEN><<<dim3((S + QT - 1) / QT, a.B * a.h), 128, smem, st>>>(tq, tkv, a);
 }
 
 void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, int B, int S, int h, int d,

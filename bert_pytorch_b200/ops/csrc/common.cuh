@@ -31,19 +31,6 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// Programmatic dependent launch (PDL): a kernel launched with launch_pdl() may become resident while its predecessor
-// in the stream is still draining; everything it does before pdl_wait() (barrier init, descriptor
-// prefetch) overlaps the predecessor's tail, pdl_wait() returns once the predecessor grid has completed and its
-// writes are visible.  pdl_trigger() lets the NEXT kernel's CTAs be scheduled as soon as every CTA of this grid has
-// started.  Both are no-ops for a kernel launched without the attribute.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-// the same for the kernels that are not persistent GEMMs; -DB200_PDL_GEMM_ONLY (A/B build) leaves only the GEMMs triggering
-__device__ __forceinline__ void pdl_trigger_small() {
-#ifndef B200_PDL_GEMM_ONLY
-  pdl_trigger();
-#endif
-}
 
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -396,24 +383,5 @@ inline int num_sms() {                   // SMs of the current device (132 on an
     B200_CUDA_CHECK(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
   }
   return n;
-}
-}  // namespace b200
-
-// launch with the programmatic-stream-serialization attribute (see pdl_wait above); B200_PDL=0 launches plainly
-#include <utility>
-namespace b200 {
-inline bool pdl_enabled() {
-  static const bool on = []() { const char* e = getenv("B200_PDL"); return e && e[0] == '1'; }();   // opt-in until measured
-  return on;
-}
-template <typename... KArgs, typename... Args>
-inline void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;     // no attribute at all unless PDL is on
-  B200_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, KArgs(std::forward<Args>(args))...));
 }
 }  // namespace b200

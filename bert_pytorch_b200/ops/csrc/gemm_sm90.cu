@@ -684,8 +684,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
-  pdl_trigger();
   constexpr int BK = FP8 ? 128 : 64;             // elements along K per stage
 
   if (wg == 0) {
@@ -910,7 +908,7 @@ static void launch(const GemmCall& c, cudaStream_t st) {
   p.timeline = p.units <= g_timeline_units ? g_timeline : nullptr;
 #endif
   const int grid = p.units < num_sms() ? p.units : num_sms();       // persistent: one CTA per SM walks the units
-  launch_pdl(kern, dim3(grid), dim3(NUM_THREADS), SMEM, st, ta, tb, to, tres, p);
+  kern<<<grid, NUM_THREADS, SMEM, st>>>(ta, tb, to, tres, p);
 }
 
 // fp8: bring an MN-major operand ([K][ld], the M or N index contiguous) into the K-major form [MN][Kp]

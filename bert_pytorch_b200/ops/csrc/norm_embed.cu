@@ -134,8 +134,6 @@ ln_fwd_row_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__
                   float eps, int h, const Fp8Out f8) {
   const int H = TAIL ? h : CHUNKS * 256;
   __shared__ float4 sg[CHUNKS][2][32], sb[CHUNKS][2][32];   // [chunk][half of the lane's 8 columns][lane]
-  pdl_trigger_small();
-  pdl_wait();
   for (int i = threadIdx.x; i < CHUNKS * 64; i += blockDim.x) {
     const int c = i >> 6, hf = (i >> 5) & 1, l = i & 31;
     const int col = c * 256 + l * 8 + hf * 4;
@@ -228,8 +226,6 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
   const int H = TAIL ? h : WPR * 256;
   __shared__ float2 xchg[GROUPS][2][WPR];
   __shared__ float comb[GROUPS - 1 > 0 ? GROUPS - 1 : 1][3][WPR * 256];
-  pdl_trigger_small();
-  pdl_wait();
   const unsigned long long seed = thresh16 != 0 ? seed_in.value() : 0ull;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int group = warp / WPR, wi = warp % WPR;
@@ -386,8 +382,6 @@ ln_bwd3_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
 __global__ void __launch_bounds__(256)
 colsum_finalize_kernel(const float* __restrict__ partial, int nblocks, int H, float* dgamma, float* dbeta,
                        float* dbias) {
-  pdl_trigger_small();
-  pdl_wait();
   const int qn = blockIdx.y;
   float* dst = qn == 0 ? dgamma : (qn == 1 ? dbeta : dbias);
   if (dst == nullptr) return;
@@ -418,8 +412,6 @@ colsum_finalize_kernel(const float* __restrict__ partial, int nblocks, int H, fl
 __global__ void __launch_bounds__(256) colsum_bf16_kernel(const __nv_bfloat16* __restrict__ x, int M, int N, int ld,
                                                          float* __restrict__ out) {
   // block: 32 column-groups (8 cols each = 256 columns) x 8 row lanes
-  pdl_trigger_small();
-  pdl_wait();
   const int cg = threadIdx.x & 31, rl = threadIdx.x >> 5;
   const int col = blockIdx.x * 256 + cg * 8;
   float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -1034,8 +1026,7 @@ void layer_norm_fwd(const void* x, const float* gamma, const float* beta, void* 
                                                                 : ln_fwd_row_kernel<8, true, true>;
   int g = (M + 7) / 8;
   if (g > num_sms() * 4) g = num_sms() * 4;
-  launch_pdl(k, dim3(g), dim3(256), 0, st, (const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, M, eps,
-             H, f8);
+  k<<<g, 256, 0, st>>>((const __nv_bfloat16*)x, gamma, beta, (__nv_bfloat16*)y, mean, rstd, M, eps, H, f8);
 }
 
 // Rows per block of the LN backward: 256 threads, WPR = 8 / groups warps per row (the H = 768 kernel: 3 x 2 warps).
@@ -1072,13 +1063,12 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
         : wpr == 4 ? ln_bwd3_kernel<4, 2, true, true> : ln_bwd3_kernel<8, 1, true, true>;
   }
   const int grid = ln_bwd_grid(M, H);
-  launch_pdl(k, dim3(grid), dim3(wpr * ln_bwd_groups(H) * 32), 0, st, (const __nv_bfloat16*)dy,
-             (const __nv_bfloat16*)x, mean, rstd, gamma, (__nv_bfloat16*)dx, (__nv_bfloat16*)dxd, workspace, M, seed,
-             drop_stream, th, sc, keep_mask, H, in_stream, f8);
+  k<<<grid, wpr * ln_bwd_groups(H) * 32, 0, st>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x, mean, rstd, gamma,
+                                                  (__nv_bfloat16*)dx, (__nv_bfloat16*)dxd, workspace, M, seed,
+                                                  drop_stream, th, sc, keep_mask, H, in_stream, f8);
   // deterministic: one slice, so every column is finished by a plain += in a fixed order
-  launch_pdl(colsum_finalize_kernel, dim3((H + 31) / 32, 3, deterministic ? 1 : 8), dim3(256), 0, st,
-             (const float*)workspace, grid, H,
-             dgamma, dbeta, dxd ? dbias : (float*)nullptr);
+  colsum_finalize_kernel<<<dim3((H + 31) / 32, 3, deterministic ? 1 : 8), 256, 0, st>>>(workspace, grid, H, dgamma, dbeta,
+                                                                                       dxd ? dbias : nullptr);
 }
 
 // Keep bits of one hidden-dropout site, one byte per 8 elements ([M][N / 8], bit t of byte j = element 8 j + t kept):
@@ -1087,7 +1077,6 @@ void layer_norm_bwd(const void* dy, const void* x, const float* mean, const floa
 // meanwhile) and instead of being regenerated by the LayerNorm backward.
 __global__ void __launch_bounds__(256) dropout_mask_kernel(unsigned int* __restrict__ out, long long n_words, Seed seed_in,
                                                            unsigned int stream, unsigned int thresh16) {
-  pdl_trigger_small();
   const PhiloxKeys keys = philox_keys(seed_in.value());
   const uint32_t T = thresh16 << 16;
   for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w < n_words; w += (long long)gridDim.x * blockDim.x) {
@@ -1108,12 +1097,12 @@ void dropout_mask(void* out, long long n_elems, Seed seed, unsigned int stream, 
   const long long n_words = n_elems / 32;
   long long g = (n_words + 255) / 256;
   if (g > num_sms() * 16) g = num_sms() * 16;
-  if (g > 0) launch_pdl(dropout_mask_kernel, dim3((unsigned)g), dim3(256), 0, st, (unsigned int*)out, n_words, seed, stream, th);
+  if (g > 0) dropout_mask_kernel<<<(unsigned)g, 256, 0, st>>>((unsigned int*)out, n_words, seed, stream, th);
 }
 
 void colsum_bf16(const void* x, int M, int N, int ld, float* out, cudaStream_t st) {
   dim3 grid((N + 255) / 256, M >= 4096 ? 64 : (M >= 512 ? 16 : 1));
-  launch_pdl(colsum_bf16_kernel, grid, dim3(256), 0, st, (const __nv_bfloat16*)x, M, N, ld, out);
+  colsum_bf16_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, M, N, ld, out);
 }
 
 void gelu_fwd(const void* x, void* y, long long n, Fp8Out f8, cudaStream_t st) {

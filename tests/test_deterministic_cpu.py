@@ -1,6 +1,6 @@
 """Deterministic mode, the switches (no GPU needed): ``ops.api.deterministic()`` under the environment variable and
-under torch's flag, ``--deterministic`` and the JSON key on the three runners, and the mode's place in the CUDA-graph
-key of ``FusedPretrainer``."""
+under torch's flag, ``--deterministic`` and the JSON key on the three runners, the mode's place in the CUDA-graph
+key of ``FusedPretrainer``, and the [CLS] row indices that captured graphs keep reading."""
 import json
 import os
 
@@ -129,3 +129,24 @@ def test_graph_key_holds_the_mode(monkeypatch):
         pt.forward_backward(t, t, t, t, torch.zeros(2, dtype=torch.int32))
     assert len(keys) == 2 and keys[0] != keys[1]
     assert keys[0][-2] is False and keys[1][-2] is True           # the last entry is the token bucket
+
+
+def test_cls_rows_stay_one_tensor_per_batch_shape():
+    """A captured graph reads the padded [CLS] row indices of its batch shape through a raw pointer: requesting other
+    shapes must neither replace nor free that tensor.  A packed batch brings its own indices."""
+    from types import SimpleNamespace
+
+    from bert_pytorch_b200 import BertConfig
+    from bert_pytorch_b200.models import BertForPreTraining
+    from bert_pytorch_b200.models.fused import FusedPretrainer
+    cfg = BertConfig(vocab_size_or_config_json_file=64, hidden_size=64, num_hidden_layers=1, num_attention_heads=1,
+                     intermediate_size=128, max_position_embeddings=16)
+    pt = FusedPretrainer(BertForPreTraining(cfg))
+    cpu = torch.device("cpu")
+    first = pt._cls_rows(None, 4, 16, cpu)
+    assert first.dtype == torch.int32 and first.tolist() == [0, 16, 32, 48]
+    for B, S in ((3, 16), (4, 8), (8, 16)):
+        assert pt._cls_rows(None, B, S, cpu).tolist() == [b * S for b in range(B)]
+    assert pt._cls_rows(None, 4, 16, cpu) is first
+    pk = SimpleNamespace(cls_rows=torch.tensor([0, 5, 9], dtype=torch.int32))
+    assert pt._cls_rows(pk, 3, 16, cpu) is pk.cls_rows

@@ -2,10 +2,9 @@
 sums in a scheduling-dependent order by default gives the same bits on a second call, the fixed-order forms still meet
 the fp64 reference tests of their kernels, and whole training steps -- padded and unpadded, S = 128 and 512, NSP,
 activation checkpointing, fp8 operands -- repeat bit for bit, also across the scheduling choices (weight-gradient side
-stream, CUDA-graph replay, programmatic dependent launch) that only change when kernels run."""
+stream, CUDA-graph replay) that only change when kernels run, and a replayed graph repeats its loss after batches of
+another shape."""
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -15,8 +14,6 @@ import test_gpu_optim_loss as optim_ref
 from test_gpu_pretrain_unpad import _batch, _grad_errors, _grads, _model, _tokens
 
 pytestmark = pytest.mark.gpu
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture
@@ -356,25 +353,26 @@ def test_scheduling_does_not_change_the_bits(det, unpad):
         _same(replay, eager, "graph replay")
 
 
-_PDL_SCRIPT = r"""
-import sys, torch
-sys.path[:0] = [{root!r}, {tests!r}]
-from test_gpu_deterministic import _train
-out = _train(512, True, steps=2)
-torch.save({{k: v.cpu() for k, v in out.items()}}, sys.argv[1])
-"""
+def test_nsp_graph_replays_alike_after_a_batch_of_another_size(det):
+    """The graph of a batch shape reads the [CLS] row indices of the NSP head through the pointer it was captured with:
+    a batch of another size (the short last batch of an epoch) must leave that tensor alive.  Dropout 0 and no
+    optimizer step, so every replay of the same batch gives the same loss."""
+    S = 128
+    model, arena, pt = _model(S=S)
+    assert pt.use_graphs and pt.has_nsp
+    full = _batch(8, S, [S, S // 3, 1, 0, S - 1, 65, S // 2 + 3, 100], seed=1)
+    short = _batch(5, S, [S, 3, 64, 0, 99], seed=2)
 
-
-def test_programmatic_dependent_launch_does_not_change_the_bits(tmp_path):
-    """B200_PDL is read once per process: one process per setting."""
-    script = _PDL_SCRIPT.format(root=ROOT, tests=os.path.join(ROOT, "tests"))
-    res = []
-    for pdl in ("0", "1"):
-        env = dict(os.environ, B200_PDL=pdl, B200_DETERMINISTIC="1")
-        path = str(tmp_path / f"pdl{pdl}.pt")
-        subprocess.run([sys.executable, "-c", script, path], env=env, check=True, cwd=ROOT)
-        res.append(torch.load(path))
-    _same(res[0], res[1], "PDL 0 / 1")
+    def captured(batch):                             # the eager calls, the capture, then one more replay
+        losses = [pt.forward_backward(*batch).clone() for _ in range(pt.graph_warmup + 2)]
+        torch.cuda.synchronize()
+        return losses[-1]
+    before = captured(full)
+    captured(short)
+    assert sum("graph" in e for e in pt._graphs.values()) == 2
+    after = pt.forward_backward(*full).clone()
+    torch.cuda.synchronize()
+    assert torch.equal(before, after), (before.item(), after.item())
 
 
 def test_deterministic_mode_agrees_with_the_default_mode(monkeypatch):

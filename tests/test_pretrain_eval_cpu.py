@@ -172,7 +172,9 @@ def test_oracle_evaluate_ties_go_to_the_lowest_index():
 
 def test_two_rank_world_matches_one_rank(tmp_path):
     s = _set(_shards(tmp_path / "d"), n=24)          # each rank's batches are batches of the one-rank run: equal rows
-    model = _model()
+    # the ranks are threads sharing one model: in training mode, one rank's evaluate could switch the training flag
+    # (and with it dropout) back on while the other rank's forward runs
+    model = _model().eval()
 
     def run(comm):
         acc = torch.zeros(6, dtype=torch.float64)
