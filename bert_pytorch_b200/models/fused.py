@@ -555,20 +555,21 @@ class FusedEncoderEngine:
                               self.g(pre + "attention.output.dense.weight"), dyq=q[0] if q else None)
         # ---- attention core
         dqkv_q = None
+        d_bqkv = self._qkv(l, A.flat_grad, "bias")           # the attention backward adds the QKV bias gradient
         if sv.pk is not None:
             d_qkv = K.attention_bwd(ls.qkv, None, ls.ctx, d_ctx, ls.lse, self.heads, p_drop=pa, seed=seed,
-                                    stream=_stream(l, SITE_ATTN_PROB), cu_seqlens=sv.pk.cu_seqlens, S=sv.S)
+                                    stream=_stream(l, SITE_ATTN_PROB), cu_seqlens=sv.pk.cu_seqlens, S=sv.S, dbias=d_bqkv)
         else:
             d_qkv, *q = _as_tuple(K.attention_bwd(ls.qkv.view(sv.B, sv.S, 3 * H), sv.seqlens, ls.ctx.view(sv.B, sv.S, H),
                                                   d_ctx.view(sv.B, sv.S, H), ls.lse, self.heads, p_drop=pa, seed=seed,
-                                                  stream=_stream(l, SITE_ATTN_PROB), fp8=self._side(f"{l}.d_qkv")))
+                                                  stream=_stream(l, SITE_ATTN_PROB), fp8=self._side(f"{l}.d_qkv"),
+                                                  dbias=d_bqkv))
             d_qkv = d_qkv.view(M, 3 * H)
             dqkv_q = q[0].view(M, 3 * H) if q else None
         if kfac is not None:
             for j, nm in enumerate(("query", "key", "value")):
                 kfac.tap(self.prefix + pre + "attention.self." + nm, ls.x, d_qkv[:, j * H:(j + 1) * H])
         # ---- QKV projection
-        K.colsum_accumulate(d_qkv, self._qkv(l, A.flat_grad, "bias"))
         d = self._lin_bwd(l, "d_qkv", "x", "wqkv", d_qkv, ls.x_op, self._qkv(l, A.flat_shadow, "weight"),
                           self._qkv(l, A.flat_grad, "weight"), dyq=dqkv_q, epi=K.EPI_ADD, res=d_pre1)
         self._wgrad_layer_done()

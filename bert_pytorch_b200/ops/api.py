@@ -491,20 +491,28 @@ def attention_fwd(qkv: torch.Tensor, seqlens: Optional[torch.Tensor], heads: int
 
 
 def attention_bwd(qkv, seqlens, ctx, dctx, lse, heads: int, *, p_drop=0.0, seed=0, stream=0, fp8=None,
-                  cu_seqlens: Optional[torch.Tensor] = None, S: Optional[int] = None):
+                  cu_seqlens: Optional[torch.Tensor] = None, S: Optional[int] = None,
+                  dbias: Optional[torch.Tensor] = None, _general: bool = False):
     """Both forms as :func:`attention_fwd`.  ``fp8=(meta, site)``: the kernels also write the fp8 copy of dqkv ->
-    (dqkv, q)."""
+    (dqkv, q).  ``dbias`` (fp32 [3H], the QKV bias gradient) += the column sums of dqkv (:func:`colsum_accumulate`).
+    S <= 128 runs the one-pass kernel (no delta or dQ accumulation buffers); ``_general`` runs the multi-block path
+    there too (for tests that compare the two)."""
     B, S, rows, H = _attn_shape(qkv, seqlens, cu_seqlens, S)
     dqkv = torch.empty_like(qkv)
-    delta = torch.empty(B, heads, S, dtype=torch.float32, device=qkv.device)
-    # deterministic mode with more than one 128-key block: one dQ slice per key block, summed in key-block order
     det = deterministic()
-    slices = (S + 127) // 128 if det and S > 128 else 1
-    dq_acc = torch.empty(slices, rows, H, dtype=torch.float32, device=qkv.device)
+    onepass = S <= 128 and not _general
+    delta = dq_acc = None
+    if not onepass:
+        delta = torch.empty(B, heads, S, dtype=torch.float32, device=qkv.device)
+        # deterministic mode with more than one 128-key block: one dQ slice per key block, summed in key-block order
+        slices = (S + 127) // 128 if det and S > 128 else 1
+        dq_acc = torch.empty(slices, rows, H, dtype=torch.float32, device=qkv.device)
     q, rec, e5 = _fp8_side(fp8, dqkv)
     extension().attention_bwd(qkv, seqlens, ctx, dctx, lse, dqkv, delta, dq_acc, heads, 1.0 / math.sqrt(H // heads), p_drop,
-                              seed, stream, q, rec, e5, cu_seqlens, S, det)
-    _count(2)
+                              seed, stream, q, rec, e5, cu_seqlens, S, det, _general)
+    _count(1 if onepass else 2)
+    if dbias is not None:
+        colsum_accumulate(dqkv.view(-1, 3 * H), dbias)
     return dqkv if fp8 is None else (dqkv, q)
 
 

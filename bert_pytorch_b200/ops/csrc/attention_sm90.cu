@@ -15,6 +15,8 @@
 //           formed in registers; dQ += dS K takes dS from registers; P~ and dS pass through shared memory once and
 //           are read MN-major for dV += P~^T dO and dK += dS^T Q.  dQ is reduced across key blocks with fp32 reductions
 //           into dq_acc and converted to bf16 by attn_dq_convert_kernel; delta = <dO, O> comes from attn_delta_kernel.
+//           S <= 128 (one key block) runs attn_bwd_onepass_kernel instead: the same per-block math in a persistent
+//           CTA per (batch, head) item, with delta and the dQ sum inside.
 // Varlen (VARLEN = true): qkv is packed [T, 3H] and ctx / dctx / dq_acc are [T, H]; sequence b owns rows
 // cu_seqlens[b] .. cu_seqlens[b + 1] (passed in AttnArgs::seqlens).  S is the padded length: it sizes the grid and is
 // the stride of the dropout counter, so the keep decisions equal the padded kernel's for the same batch.  lse and
@@ -97,14 +99,16 @@ __device__ __forceinline__ void regroup8(const float* acc4, int h, float (&f)[8]
   }
 }
 
-// Store a [64 rows x 64 columns] accumulator tile as bf16 (16 bytes per lane and row half) + optional fp8 copy.
-// row_lo: this lane's first row inside the tile; n_valid: rows of the tile that exist; dst: element (0, 0) of the tile.
-__device__ __forceinline__ void store_tile64(const float (&acc)[32], float mul_lo, float mul_hi, int row_lo, int n_valid,
+// Store NU 32-column halves of a [64 rows x 64 columns] accumulator tile (acc: 16 NU fragment values) as bf16
+// (16 bytes per lane and row half) + optional fp8 copy.  row_lo: this lane's first row inside the tile; n_valid: rows of
+// the tile that exist; dst: element (0, 0) of the first half.
+template <int NU>
+__device__ __forceinline__ void store_cols64(const float* acc, float mul_lo, float mul_hi, int row_lo, int n_valid,
                                              __nv_bfloat16* dst, size_t ld, const Fp8Out& f8, size_t f8_off, float qscale,
                                              float& amax) {
   const int c = threadIdx.x & 3;
 #pragma unroll
-  for (int u = 0; u < 2; ++u) {
+  for (int u = 0; u < NU; ++u) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float f[8];
@@ -121,6 +125,13 @@ __device__ __forceinline__ void store_tile64(const float (&acc)[32], float mul_l
       }
     }
   }
+}
+
+// the whole tile
+__device__ __forceinline__ void store_tile64(const float (&acc)[32], float mul_lo, float mul_hi, int row_lo, int n_valid,
+                                             __nv_bfloat16* dst, size_t ld, const Fp8Out& f8, size_t f8_off, float qscale,
+                                             float& amax) {
+  store_cols64<2>(acc, mul_lo, mul_hi, row_lo, n_valid, dst, ld, f8, f8_off, qscale, amax);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -531,6 +542,255 @@ attn_dq_convert_sliced_kernel(const float* __restrict__ acc, __nv_bfloat16* __re
 }
 
 // ------------------------------------------------------------------------------------------------
+// one-pass backward (S <= 128: one key block holds every key of a sequence)
+// ------------------------------------------------------------------------------------------------
+// attn_bwd_onepass_kernel: persistent; CTA x walks the (batch, head) items x, x + gridDim.x, ...  The CTA of an item
+// sees every query and key of its head, so the whole backward is one pass:
+//  - delta = <dO, O> of a query block from its dO and O tiles in shared memory, with attn_delta_kernel's arithmetic
+//    (same 8-column partial sums and contraction, same xor 1, 2, 4 combine), so it is bit-identical;
+//  - the two warpgroups' dQ partials are summed through shared memory as 0 + a + b (the value the fp32 reductions
+//    into a zeroed dq_acc produce, signed zeros included) and stored as bf16 into the q slots of dqkv.
+// Loads run ahead of the MMAs: K / V are double buffered per item, and Q | dO | O per query block ("job"), so while
+// an item computes, the K / V of the next item and the first query block of the next item are in flight.
+constexpr int ATT_OP_SMEM_TILES = 2 * 32768 + 3 * 2 * 8192 + 2 * 16384;   // K|V x2, Q / dO / O x2, P~ / dS
+constexpr int ATT_OP_SMEM = ATT_OP_SMEM_TILES + 1024 + 64 + 64 * 4;
+
+template <bool VARLEN>
+__device__ __forceinline__ void onepass_item(const AttnArgs& p, int it, int& row0, int& nrows) {
+  const int b = it / p.h;
+  if constexpr (VARLEN) {
+    row0 = p.seqlens[b];
+    nrows = min(p.seqlens[b + 1] - row0, p.S);          // rows (queries = keys) of the sequence; 0: nothing to do
+  } else {
+    row0 = b * p.S;
+    nrows = p.S;                                        // every row of a padded sequence gets dQ, dK and dV
+  }
+}
+
+template <bool VARLEN>
+__device__ __forceinline__ int onepass_next(const AttnArgs& p, int it) {   // the next item of this CTA with rows
+  const int n = p.B * p.h;
+  for (it += gridDim.x; VARLEN && it < n; it += gridDim.x) {
+    int r0, nr;
+    onepass_item<VARLEN>(p, it, r0, nr);
+    if (nr > 0) break;
+  }
+  return it;
+}
+
+template <bool VARLEN>
+__global__ void __launch_bounds__(ATT_BWD_THREADS, 1)
+attn_bwd_onepass_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
+                        const __grid_constant__ CUtensorMap tmap_do, const __grid_constant__ CUtensorMap tmap_o,
+                        const AttnArgs p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sKV = smem;                       // 2 stages x (K 16 KB | V 16 KB); warpgroup w reads key rows [64 w, 64 w + 64)
+  uint8_t* sQ = smem + 65536;                // 2 stages x 8 KB
+  uint8_t* sDO = sQ + 16384;                 // 2 stages x 8 KB
+  uint8_t* sO = sDO + 16384;                 // 2 stages x 8 KB
+  uint8_t* sP = sO + 16384;                  // 2 warpgroups x 8 KB: P~, then this warpgroup's dQ half for the other one
+  uint8_t* sDS = sP + 16384;                 // 2 warpgroups x 8 KB: dS
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ATT_OP_SMEM_TILES);   // [0], [1]: K / V stages, [2], [3]: jobs
+  float* sDelta = reinterpret_cast<float*>(bars + 8);                      // [64] delta of the current query block
+
+  const int nitems = p.B * p.h;
+  int first = blockIdx.x;
+  if (VARLEN && first < nitems) {
+    int r0, nr;
+    onepass_item<VARLEN>(p, first, r0, nr);
+    if (nr == 0) first = onepass_next<VARLEN>(p, first);
+  }
+  if (first >= nitems) return;                          // CTA uniform, before any mbarrier or TMA work
+
+  // producer state (thread 0): the next item whose K / V to load, the next job (item, query block) whose Q / dO / O
+  int kv_it = first, kv_n = 0, job_it = first, job_qb = 0, job_n = 0;
+  auto issue_kv = [&]() {
+    if (kv_it >= nitems) return;
+    int r0, nr;
+    onepass_item<VARLEN>(p, kv_it, r0, nr);
+    const int head = kv_it % p.h, st = kv_n & 1;
+    mbar_arrive_expect_tx(&bars[st], 32768);
+    tma_load_2d(sKV + st * 32768, &tmap_kv, &bars[st], p.H + head * HD, r0);
+    tma_load_2d(sKV + st * 32768 + 16384, &tmap_kv, &bars[st], 2 * p.H + head * HD, r0);
+    ++kv_n;
+    kv_it = onepass_next<VARLEN>(p, kv_it);
+  };
+  auto issue_job = [&]() {
+    if (job_it >= nitems) return;
+    int r0, nr;
+    onepass_item<VARLEN>(p, job_it, r0, nr);
+    const int head = job_it % p.h, st = job_n & 1, row = r0 + job_qb * QT;
+    mbar_arrive_expect_tx(&bars[2 + st], 3 * 8192);
+    tma_load_2d(sQ + st * 8192, &tmap_q, &bars[2 + st], head * HD, row);
+    tma_load_2d(sDO + st * 8192, &tmap_do, &bars[2 + st], head * HD, row);
+    tma_load_2d(sO + st * 8192, &tmap_o, &bars[2 + st], head * HD, row);
+    ++job_n;
+    if (++job_qb * QT >= nr) {
+      job_qb = 0;
+      job_it = onepass_next<VARLEN>(p, job_it);
+    }
+  };
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_q);
+    tma_prefetch_desc(&tmap_kv);
+    tma_prefetch_desc(&tmap_do);
+    tma_prefetch_desc(&tmap_o);
+    for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    issue_kv(); issue_kv();
+    issue_job(); issue_job();
+  }
+
+  const int wg = threadIdx.x >> 7, tw = threadIdx.x & 127;
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, c = lane & 3;
+  const int r_lo = warp * 16 + (lane >> 2);
+  const int key0 = wg * 64;                  // first key of this warpgroup
+  const float c_scale = p.scale * LOG2E;
+  const bool drop = p.thresh16 != 0;
+  const PhiloxKeys keys = philox_keys(drop ? p.seed.value() : 0ull);
+  uint8_t* myP = sP + wg * 8192;
+  uint8_t* myDS = sDS + wg * 8192;
+  const uint32_t ap = smem_u32(myP), ads = smem_u32(myDS);
+  const float* otherDq = reinterpret_cast<const float*>(sP + (wg ^ 1) * 8192);
+  float amax = 0.f;
+  const float qscale = p.f8.q ? p.f8.meta[1] : 0.f;
+  const size_t ld = (size_t)3 * p.H;
+  int j = 0;                                 // jobs done by this CTA
+
+  for (int it = first, n = 0; it < nitems; it = onepass_next<VARLEN>(p, it), ++n) {
+    const int bh = it, head = it % p.h;
+    int row0, q_end;
+    onepass_item<VARLEN>(p, it, row0, q_end);
+    int seqlen = q_end;                      // valid keys
+    if constexpr (!VARLEN) {
+      seqlen = min(p.seqlens[it / p.h], p.S);
+      if (seqlen <= 0) seqlen = p.S;                    // a fully masked sequence attends to every key
+    }
+    const int nqb = (q_end + QT - 1) / QT;
+    const uint32_t ak = smem_u32(sKV + (n & 1) * 32768) + wg * 8192, av = ak + 16384;
+    float dv[32], dk[32];
+#pragma unroll
+    for (int t = 0; t < 32; ++t) dv[t] = dk[t] = 0.f;
+
+    mbar_wait_mma(&bars[n & 1], (n >> 1) & 1);
+    for (int i = 0; i < nqb; ++i, ++j) {
+      const int st = j & 1;
+      mbar_wait_mma(&bars[2 + st], (j >> 1) & 1);
+      {                                      // delta of the 64 rows: 8 lanes per row, 8 columns per lane
+        const uint8_t* o_t = sO + st * 8192;
+        const uint8_t* d_t = sDO + st * 8192;
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const int r = (threadIdx.x >> 3) + 32 * k, sub = threadIdx.x & 7;
+          const uint32_t off = r * 128 + ((sub ^ (r & 7)) << 4);
+          const uint4 a = *reinterpret_cast<const uint4*>(o_t + off), d = *reinterpret_cast<const uint4*>(d_t + off);
+          const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, dw[4] = {d.x, d.y, d.z, d.w};
+          float s = 0.f;
+#pragma unroll
+          for (int t = 0; t < 4; ++t) {          // attn_delta_kernel's contraction: s + fma(x.x, y.x, x.y * y.y)
+            const float2 x = unpack_bf16(aw[t]), y = unpack_bf16(dw[t]);
+            s = __fadd_rn(s, __fmaf_rn(x.x, y.x, __fmul_rn(x.y, y.y)));
+          }
+          s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 1));
+          s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 2));
+          s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, 4));
+          if (sub == 0) sDelta[r] = s;
+        }
+      }
+      __syncthreads();
+      const uint32_t aq = smem_u32(sQ + st * 8192), ado = smem_u32(sDO + st * 8192);
+      float s[32], dp[32];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < HD / 16; ++kk) {
+        WgmmaBf16SS<64, 0, 0>::mma(s, wgmma_desc_sw128(aq + kk * 32, 16, 1024), wgmma_desc_sw128(ak + kk * 32, 16, 1024), kk > 0);
+        WgmmaBf16SS<64, 0, 0>::mma(dp, wgmma_desc_sw128(ado + kk * 32, 16, 1024), wgmma_desc_sw128(av + kk * 32, 16, 1024), kk > 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      wgmma_fence_regs(dp);
+      uint32_t dsp[2][8];                    // dS of this lane, bf16 pairs: [row half][key group]
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r_lo + 8 * h, q = i * QT + r;
+        const bool q_ok = q < q_end;
+        const float lse2 = q_ok ? __ldg(p.lse + (size_t)bh * p.S + q) * LOG2E : 0.f;
+        const float dlt = q_ok ? sDelta[r] : 0.f;
+        uint32_t w[8];
+        if (drop) {
+          const uint64_t erow = ((uint64_t)bh * p.S + (uint64_t)q) * (uint64_t)p.S;
+          draw_row<8>(w, keys, (erow + (uint64_t)key0) >> 3, p.stream);
+        }
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          const int key = key0 + 8 * g + 2 * c;
+          const float pr0 = (q_ok && key < seqlen) ? ex2_approx(fmaf(s[4 * g + 2 * h], c_scale, -lse2)) : 0.f;
+          const float pr1 = (q_ok && key + 1 < seqlen) ? ex2_approx(fmaf(s[4 * g + 2 * h + 1], c_scale, -lse2)) : 0.f;
+          bool ka = true, kb2 = true;
+          if (drop) keep_pair(w[g], p.thresh16, ka, kb2);
+          const float dp0 = ka ? dp[4 * g + 2 * h] * p.inv_keep : 0.f;
+          const float dp1 = kb2 ? dp[4 * g + 2 * h + 1] * p.inv_keep : 0.f;
+          const uint32_t pd = pack_bf16(ka ? pr0 * p.inv_keep : 0.f, kb2 ? pr1 * p.inv_keep : 0.f);
+          const uint32_t ds = pack_bf16(pr0 * (dp0 - dlt) * p.scale, pr1 * (dp1 - dlt) * p.scale);
+          dsp[h][g] = ds;
+          *reinterpret_cast<uint32_t*>(myP + tile_pair_offset(r, g, c)) = pd;
+          *reinterpret_cast<uint32_t*>(myDS + tile_pair_offset(r, g, c)) = ds;
+        }
+      }
+      fence_proxy_async();                   // generic-proxy smem writes -> visible to wgmma (async proxy)
+      asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory");
+      float dq[32];
+      wgmma_fence_regs(dv);
+      wgmma_fence_regs(dk);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < QT / 16; ++kk) { // reduction over the 64 queries: P~ / dS and dO / Q all read MN-major
+        WgmmaBf16SS<64, 1, 1>::mma(dv, wgmma_desc_sw128(ap + kk * 2048, 8192, 1024), wgmma_desc_sw128(ado + kk * 2048, 8192, 1024), 1);
+        WgmmaBf16SS<64, 1, 1>::mma(dk, wgmma_desc_sw128(ads + kk * 2048, 8192, 1024), wgmma_desc_sw128(aq + kk * 2048, 8192, 1024), 1);
+      }
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {       // dQ (partial: this warpgroup's 64 keys) = dS K
+        const uint32_t a[4] = {dsp[0][2 * kk], dsp[1][2 * kk], dsp[0][2 * kk + 1], dsp[1][2 * kk + 1]};
+        WgmmaBf16RS<64, 1>::mma(dq, a, wgmma_desc_sw128(ak + kk * 2048, 8192, 1024), kk > 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(dv);
+      wgmma_fence_regs(dk);
+      wgmma_fence_regs(dq);
+      // dQ: warpgroup w stores columns [32 w, 32 w + 32).  It hands the other half of its partial to the other
+      // warpgroup through its own P~ buffer (its MMAs are done with it), fragment-major so the reads match lanes.
+      float* give = reinterpret_cast<float*>(myP);
+      float mine[16];
+#pragma unroll
+      for (int k = 0; k < 16; ++k) {
+        give[k * 128 + tw] = wg ? dq[k] : dq[16 + k];
+        mine[k] = wg ? dq[16 + k] : dq[k];
+      }
+      __syncthreads();
+#pragma unroll
+      for (int k = 0; k < 16; ++k) mine[k] = __fadd_rn(__fadd_rn(0.f, mine[k]), otherDq[k * 128 + tw]);
+      const size_t q_off = (size_t)(row0 + i * QT) * ld + head * HD + wg * 32;
+      store_cols64<1>(mine, 1.f, 1.f, r_lo, q_end - i * QT, p.dqkv + q_off, ld, p.f8, q_off, qscale, amax);
+      __syncthreads();                       // both warpgroups are done with stage st and with the P~ buffers
+      if (threadIdx.x == 0) issue_job();
+    }
+    // dK -> k slots, dV -> v slots of dqkv (rows = keys of this warpgroup)
+    const size_t k_off = (size_t)(row0 + key0) * ld + p.H + head * HD;
+    store_tile64(dk, 1.f, 1.f, r_lo, q_end - key0, p.dqkv + k_off, ld, p.f8, k_off, qscale, amax);
+    store_tile64(dv, 1.f, 1.f, r_lo, q_end - key0, p.dqkv + k_off + p.H, ld, p.f8, k_off + p.H, qscale, amax);
+    __syncthreads();                         // K / V stage n & 1 is free
+    if (threadIdx.x == 0) issue_kv();
+  }
+  if (p.f8.q) fp8_amax_commit(p.f8, amax);
+}
+
+// ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
 // head_dim 64, S <= 512 and S % 8 == 0 are checked by the bindings
@@ -568,6 +828,27 @@ void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, i
 }
 
 template <bool VARLEN>
+static void launch_bwd_onepass(const void* qkv, const void* ctx, const void* dctx, const AttnArgs& a, long long rows,
+                               cudaStream_t st) {
+  const int H = a.H;
+  CUtensorMap tq = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, QT);
+  CUtensorMap tkv = make_tmap_2d_bf16(qkv, 3 * H, (uint64_t)rows, 3 * H, 64, KT);
+  CUtensorMap td = make_tmap_2d_bf16(dctx, H, (uint64_t)rows, H, 64, QT);
+  CUtensorMap to = make_tmap_2d_bf16(ctx, H, (uint64_t)rows, H, 64, QT);
+  static int resident = 0;                                // CTAs of the kernel one SM holds
+  if (resident == 0) {
+    B200_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_onepass_kernel<VARLEN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ATT_OP_SMEM));
+    B200_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, attn_bwd_onepass_kernel<VARLEN>,
+                                                                  ATT_BWD_THREADS, ATT_OP_SMEM));
+    if (resident < 1) { fprintf(stderr, "[b200] attn_bwd_onepass_kernel does not fit on an SM\n"); abort(); }
+  }
+  const long long items = (long long)a.B * a.h;
+  const int grid = (int)std::min<long long>(items, (long long)num_sms() * resident);
+  if (grid > 0) attn_bwd_onepass_kernel<VARLEN><<<grid, ATT_BWD_THREADS, ATT_OP_SMEM, st>>>(tq, tkv, td, to, a);
+}
+
+template <bool VARLEN>
 static void launch_bwd(const void* qkv, const void* ctx, const void* dctx, const AttnArgs& a, long long rows,
                        cudaStream_t st, bool deterministic) {
   const int B = a.B, S = a.S, h = a.h, H = a.H;
@@ -598,16 +879,26 @@ static void launch_bwd(const void* qkv, const void* ctx, const void* dctx, const
   else attn_dq_convert_kernel<<<g, 256, 0, st>>>(a.dq_acc, a.dqkv, rows, H, a.f8);
 }
 
+bool attention_bwd_onepass(int S, bool force_general) { return S <= KT && !force_general; }
+
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
                    Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
-                   const int* cu_seqlens, long long T, bool deterministic) {
+                   const int* cu_seqlens, long long T, bool deterministic, bool force_general) {
   AttnArgs a;
   fill_args(a, B, S, h, d, cu_seqlens ? cu_seqlens : seqlens, scale, seed, stream, p_drop);
   a.f8 = f8;
   a.lse = const_cast<float*>(lse); a.delta = delta_ws; a.dqkv = (__nv_bfloat16*)dqkv; a.dq_acc = dq_acc;
   a.ctx = (__nv_bfloat16*)const_cast<void*>(ctx);
-  if (dq_acc == nullptr) { fprintf(stderr, "[b200] attention_bwd needs a dq accumulation buffer\n"); abort(); }
+  if (attention_bwd_onepass(S, force_general)) {
+    if (cu_seqlens) launch_bwd_onepass<true>(qkv, ctx, dctx, a, T, st);
+    else launch_bwd_onepass<false>(qkv, ctx, dctx, a, (long long)B * S, st);
+    return;
+  }
+  if (dq_acc == nullptr || delta_ws == nullptr) {
+    fprintf(stderr, "[b200] attention_bwd needs delta and dq accumulation buffers\n");
+    abort();
+  }
   if (cu_seqlens) launch_bwd<true>(qkv, ctx, dctx, a, T, st, deterministic);
   else launch_bwd<false>(qkv, ctx, dctx, a, (long long)B * S, st, deterministic);
 }

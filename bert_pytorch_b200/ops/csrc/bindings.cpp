@@ -580,10 +580,11 @@ void attention_fwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor
                       a.H / (int)heads, (float)scale, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
                       mk_fp8(q8, meta8, e5m2, ctx.numel()), cur_stream(), a.cu, a.rows);
 }
+// S <= 128 runs the one-pass kernel, which needs neither delta_ws nor dq_acc, unless force_general.
 void attention_bwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor dctx, Tensor lse, Tensor dqkv,
-                   Tensor delta_ws, c10::optional<Tensor> dq_acc, int64_t heads, double scale, double p_drop, int64_t seed,
-                   int64_t stream_id, c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2,
-                   c10::optional<Tensor> cu_seqlens, int64_t S, bool deterministic) {
+                   c10::optional<Tensor> delta_ws, c10::optional<Tensor> dq_acc, int64_t heads, double scale, double p_drop,
+                   int64_t seed, int64_t stream_id, c10::optional<Tensor> q8, c10::optional<Tensor> meta8, bool e5m2,
+                   c10::optional<Tensor> cu_seqlens, int64_t S, bool deterministic, bool force_general) {
   const AttnShape a = check_attention(qkv, seqlens, lse, heads, cu_seqlens, S, q8.has_value() && q8->defined());
   check_bf16(qkv, "qkv"); check_bf16(ctx, "ctx"); check_bf16(dctx, "dctx"); check_bf16(dqkv, "dqkv");
   TORCH_CHECK(qkv.is_contiguous() && ctx.is_contiguous() && dctx.is_contiguous() && dqkv.is_contiguous(), "attention_bwd needs contiguous tensors");
@@ -592,11 +593,19 @@ void attention_bwd(Tensor qkv, c10::optional<Tensor> seqlens, Tensor ctx, Tensor
   const int slices = b200::attention_dq_slices(a.S, deterministic);
   TORCH_CHECK(!dq_acc.has_value() || !dq_acc->defined() || dq_acc->numel() >= slices * a.rows * a.H,
               "attention_bwd: dq_acc must hold ", slices, " x [rows, H] floats");
+  const bool onepass = b200::attention_bwd_onepass(a.S, force_general);
+  if (!onepass) {
+    TORCH_CHECK(delta_ws.has_value() && delta_ws->defined() && dq_acc.has_value() && dq_acc->defined(),
+                "attention_bwd: the multi-block path (S > 128 or force_general) needs delta_ws and dq_acc");
+  }
+  if (delta_ws.has_value() && delta_ws->defined())
+    TORCH_CHECK(delta_ws->scalar_type() == at::kFloat && delta_ws->numel() >= (int64_t)a.B * heads * a.S,
+                "attention_bwd: delta_ws must hold [B, heads, S] floats");
   c10::cuda::CUDAGuard guard(qkv.device());
   b200::attention_bwd(qkv.data_ptr(), a.seqlens, ctx.data_ptr(), dctx.data_ptr(), lse.data_ptr<float>(),
-                      dqkv.data_ptr(), delta_ws.data_ptr<float>(), opt_f32(dq_acc), a.B, a.S, (int)heads, a.H / (int)heads,
+                      dqkv.data_ptr(), opt_f32(delta_ws), opt_f32(dq_acc), a.B, a.S, (int)heads, a.H / (int)heads,
                       (float)scale, mk_seed(seed), (unsigned)stream_id, (float)p_drop,
-                      mk_fp8(q8, meta8, e5m2, dqkv.numel()), cur_stream(), a.cu, a.rows, deterministic);
+                      mk_fp8(q8, meta8, e5m2, dqkv.numel()), cur_stream(), a.cu, a.rows, deterministic, force_general);
 }
 
 void fused_allreduce_lamb(int64_t rank, int64_t world, bool use_multicast, std::vector<int64_t> grad_ptrs,
@@ -834,6 +843,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("dq_acc"), pybind11::arg("heads"), pybind11::arg("scale"), pybind11::arg("p_drop"),
         pybind11::arg("seed"), pybind11::arg("stream_id"), pybind11::arg("q8"), pybind11::arg("meta8"),
         pybind11::arg("e5m2"), pybind11::arg("cu_seqlens"), pybind11::arg("S"),
-        pybind11::arg("deterministic") = false);
+        pybind11::arg("deterministic") = false, pybind11::arg("force_general") = false);
   m.def("fused_allreduce_lamb", &fused_allreduce_lamb);
 }

@@ -93,7 +93,11 @@ void attention_fwd(const void* qkv, const int* seqlens, void* ctx, float* lse, i
 void attention_bwd(const void* qkv, const int* seqlens, const void* ctx, const void* dctx, const float* lse,
                    void* dqkv, float* delta_ws, float* dq_acc, int B, int S, int h, int d, float scale,
                    Seed seed, unsigned int stream, float p_drop, Fp8Out f8, cudaStream_t st,
-                   const int* cu_seqlens = nullptr, long long T = 0, bool deterministic = false);
+                   const int* cu_seqlens = nullptr, long long T = 0, bool deterministic = false,
+                   bool force_general = false);
+// Whether attention_bwd runs the one-pass kernel (S <= 128 unless force_general): it needs no delta_ws / dq_acc.  The
+// general path computes delta with attn_delta_kernel and reduces dQ through dq_acc.
+bool attention_bwd_onepass(int S, bool force_general);
 // deterministic attention_bwd: dq_acc holds attention_dq_slices(S) slices of [rows, H]
 inline int attention_dq_slices(int S, bool deterministic) { return deterministic && S > 128 ? (S + 127) / 128 : 1; }
 
