@@ -114,6 +114,14 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
   TORCH_CHECK(out.size(0) == M && out.size(1) == N, "output shape mismatch");
   TORCH_CHECK(a.stride(0) % 8 == 0 && b.stride(0) % 8 == 0, "row strides must be multiples of 8 elements");
   TORCH_CHECK(N % 8 == 0, "N must be a multiple of 8");
+  // an empty reduction launches nothing: right for the accumulate-into epilogue (out += 0), but any other epilogue
+  // would leave its output unwritten
+  TORCH_CHECK(K > 0 || epi == b200::EPI_ACCUM_F32, "gemm: K == 0 leaves the ", spec.name, " output unwritten");
+  TORCH_CHECK(block_n == 128 || block_n == 256, "gemm: block_n must be 128 or 256 (the tile widths), got ", block_n);
+  // only the fp32 accumulate-into epilogue merges K ranges (split-K); any other epilogue would ignore the split
+  TORCH_CHECK(k_splits == 1 || epi == b200::EPI_ACCUM_F32, "gemm: k_splits = ", k_splits, " needs EPI_ACCUM_F32, not ",
+              spec.name);
+  TORCH_CHECK(p_drop_is_zero(p_drop) || spec.keep_bits, "gemm: p_drop > 0 but ", spec.name, " applies no dropout");
   TORCH_CHECK(out.is_cuda() && out.stride(1) == 1, "out must be CUDA with unit inner stride");
   TORCH_CHECK(out.scalar_type() == (spec.f32_out ? at::kFloat : at::kBFloat16), "out dtype does not match the epilogue");
   TORCH_CHECK(reinterpret_cast<uintptr_t>(out.data_ptr()) % 16 == 0 && out.stride(0) % (spec.f32_out ? 4 : 8) == 0,
@@ -126,17 +134,22 @@ void gemm(Tensor a, Tensor b, Tensor out, int64_t layout, int64_t epi, c10::opti
   c.A = a.data_ptr(); c.lda = (int)a.stride(0);
   c.B = b.data_ptr(); c.ldb = (int)b.stride(0);
   c.out = out.data_ptr(); c.ldo = (int)out.stride(0);
+  // an input or output the epilogue does not read or write is refused rather than ignored
   if (aux_out.has_value() && aux_out->defined()) {
+    TORCH_CHECK(spec.aux, "aux_out is not written by ", spec.name);
     check_bf16(*aux_out, "aux_out");
+    TORCH_CHECK(aux_out->dim() == 2 && aux_out->size(0) == M && aux_out->size(1) == N, "aux_out must be [M, N]");
     TORCH_CHECK(aux_out->stride(0) == out.stride(0), "aux_out must share out's row stride");
     c.aux_out = aux_out->data_ptr();
   }
   if (bias.has_value() && bias->defined()) {
+    TORCH_CHECK(spec.bias, "bias is not read by ", spec.name);
     check_bf16(*bias, "bias");
     TORCH_CHECK(bias->numel() == N, "bias length");
     c.bias = bias->data_ptr();
   }
   if (res.has_value() && res->defined()) {
+    TORCH_CHECK(spec.res || epi == b200::EPI_ADD, "res is not read by ", spec.name);
     check_bf16(*res, "res");
     TORCH_CHECK(res->size(0) == M && res->size(1) == N && res->stride(0) % 8 == 0, "res shape");
     c.res = res->data_ptr(); c.ldr = (int)res->stride(0);

@@ -84,8 +84,8 @@ def test_layer_norm_dropout_mask_consistency():
     assert (kept_fwd ^ kept_bwd).float().mean().item() < 1e-3
 
 
-def test_dropout_keep_bits_leave_the_gemm_and_feed_layer_norm_backward():
-    """Round 2b: the hidden-dropout decisions are written by the GEMM epilogue (1 bit per element, GemmCall::mask_out)
+def test_dropout_keep_bits_leave_the_wide_gemm_and_feed_layer_norm_backward():
+    """The hidden-dropout decisions are written by the 128 x 256 GEMM epilogue (1 bit per element, GemmCall::mask_out)
     and read back by the LayerNorm backward instead of re-running Philox: the bits must describe the forward output,
     and the backward with the mask must be BITWISE the backward that regenerates it."""
     K = _api()
@@ -95,16 +95,16 @@ def test_dropout_keep_bits_leave_the_gemm_and_feed_layer_norm_backward():
     zeros_b = torch.zeros(H, device="cuda", dtype=torch.bfloat16)
     res = torch.zeros(M, H, device="cuda", dtype=torch.bfloat16)
     mask = torch.zeros(M, H // 8, dtype=torch.uint8, device="cuda")
-    fwd = K.gemm(a, w, epi=K.EPI_BIAS_DROP_RES, bias=zeros_b, res=res, p_drop=0.1, seed=77, stream=19, block_n=512,
+    fwd = K.gemm(a, w, epi=K.EPI_BIAS_DROP_RES, bias=zeros_b, res=res, p_drop=0.1, seed=77, stream=19, block_n=256,
                  mask_out=mask)
-    ref = K.gemm(a, w, epi=K.EPI_BIAS_DROP_RES, bias=zeros_b, res=res, p_drop=0.1, seed=77, stream=19, block_n=512)
+    ref = K.gemm(a, w, epi=K.EPI_BIAS_DROP_RES, bias=zeros_b, res=res, p_drop=0.1, seed=77, stream=19, block_n=256)
     assert torch.equal(fwd, ref)                                          # writing the bits does not change the output
     # the same bits from the stand-alone generator (K.dropout_mask), and the epilogue applying them instead of Philox
     gen = K.dropout_mask(M, H, 0.1, 77, 19, "cuda")
     assert torch.equal(gen, mask)
     from bert_pytorch_b200.utils import philox                   # ... and the host twin of the generator
     assert torch.equal(gen.cpu(), torch.from_numpy(philox.keep_bits(77, 19, M, H, 0.1)))
-    via = K.gemm(a, w, epi=K.EPI_BIAS_DROP_RES, bias=zeros_b, res=res, p_drop=0.1, seed=77, stream=19, block_n=512, mask_in=gen)
+    via = K.gemm(a, w, epi=K.EPI_BIAS_DROP_RES, bias=zeros_b, res=res, p_drop=0.1, seed=77, stream=19, block_n=256, mask_in=gen)
     assert torch.equal(via, ref)
     bits = ((mask.view(M, H // 8, 1) >> torch.arange(8, device="cuda", dtype=torch.uint8).view(1, 1, 8)) & 1).view(M, H).bool()
     assert abs(1.0 - bits.float().mean().item() - 0.1) < 0.01
