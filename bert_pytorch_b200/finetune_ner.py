@@ -4,6 +4,10 @@ Flags and behaviour follow the reference's run_ner.py (:19-261; SURVEY.md 2.5.7)
 ``BertForTokenClassification(config, len(labels) + 1)``, loads ``ckpt['model']`` non-strictly, Adam without
 bias correction (apex FusedAdam contract -> the fused arena kernel on CUDA), ``LambdaLR 1/(1+0.05*epoch)``,
 gradient-norm clipping, macro-F1 over labels > 0, prints validation / test loss + F1.
+With ``--bf16`` on a GPU (and a ``--max_seq_len`` the engine serves) every training step and evaluation batch runs as
+the fused sm_90a program of ``BertForTokenClassification`` (``train_step`` / ``predict``: encoder, token head, its
+dropout and the masked loss in our kernels, replayed as one CUDA graph per batch shape and token bucket); ``--unpad``
+then packs each batch on the device, with no host sync.  A short last batch is filled with inert rows (label -100).
 Fixed quirk Q23: evaluation runs the model once per batch (the reference runs it twice) and accumulates
 python floats, not tensors.
 """
@@ -116,16 +120,44 @@ def _autocast(args):
     return torch.autocast(device_type=dev, dtype=torch.bfloat16, enabled=bool(args.bf16 and args.cuda))
 
 
+def fill_batch(seqs, labels, masks, batch_size: int):
+    """A short batch (host tensors [n, S]) filled up to ``batch_size`` rows with inert ones -- one unmasked [PAD]
+    token, every label -100 -- so that one batch shape (one CUDA graph) serves the whole epoch."""
+    k = batch_size - seqs.size(0)
+    if k <= 0:
+        return seqs, labels, masks
+    fill_mask = torch.zeros((k, masks.size(1)), dtype=masks.dtype)
+    fill_mask[:, 0] = 1
+    return (torch.cat([seqs, torch.zeros((k, seqs.size(1)), dtype=seqs.dtype)]),
+            torch.cat([labels, torch.full((k, labels.size(1)), -100, dtype=labels.dtype)]),
+            torch.cat([masks, fill_mask]))
+
+
+def fused_program(model, args) -> bool:
+    """Whether training and evaluation run through the model's fused sm_90a program: ``--bf16`` on a GPU, and an
+    encoder, sequence length and label count the engine serves."""
+    if not (args.cuda and args.bf16):
+        return False
+    probe = torch.zeros(1, args.max_seq_len, dtype=torch.long, device="cuda")
+    return model.bert._can_fuse(probe) and model.num_labels <= ops.api.TOKEN_HEAD_MAX_N
+
+
 def train(model, optimizer, loader, epoch: int, args, clipper: GradientClipper) -> float:
     model.train()
     metric = Metric()
     dev = torch.device("cuda" if args.cuda else "cpu")
     for seqs, labels, masks in loader:
+        if getattr(args, "fused", False):
+            seqs, labels, masks = fill_batch(seqs, labels, masks, args.batch_size)
+            tokens = int(masks.sum())                   # on the host batch: no device sync for the unpadded bucket
         seqs, labels, masks = seqs.to(dev), labels.to(dev), masks.to(dev)
         optimizer.zero_grad()
-        with _autocast(args):
-            loss = model(seqs, token_type_ids=torch.zeros_like(masks), attention_mask=masks, labels=labels)
-        loss.backward()
+        if getattr(args, "fused", False):
+            loss = model.train_step(seqs, torch.zeros_like(masks), masks, labels, tokens=tokens)
+        else:
+            with _autocast(args):
+                loss = model(seqs, token_type_ids=torch.zeros_like(masks), attention_mask=masks, labels=labels)
+            loss.backward()
         clipper.step(model.parameters())
         optimizer.step()
         metric.update(loss.item())
@@ -140,9 +172,17 @@ def evaluate(model, loader, args) -> Tuple[float, float]:
     metric = Metric()
     preds, trues = [], []
     for seqs, labels, masks in loader:
+        n = seqs.size(0)
+        if getattr(args, "fused", False):
+            seqs, labels, masks = fill_batch(seqs, labels, masks, args.batch_size)
+            tokens = int(masks.sum())
         seqs, labels, masks = seqs.to(dev), labels.to(dev), masks.to(dev)
-        with _autocast(args):
-            logits = model(seqs, token_type_ids=torch.zeros_like(masks), attention_mask=masks)
+        if getattr(args, "fused", False):
+            logits = model.predict(seqs, torch.zeros_like(masks), masks, tokens=tokens)
+            seqs, labels, masks, logits = seqs[:n], labels[:n], masks[:n], logits[:n]
+        else:
+            with _autocast(args):
+                logits = model(seqs, token_type_ids=torch.zeros_like(masks), attention_mask=masks)
         keep = masks.view(-1) == 1
         loss = torch.nn.functional.cross_entropy(logits.view(-1, logits.size(-1)).float()[keep], labels.view(-1)[keep])
         metric.update(loss.item())
@@ -169,6 +209,7 @@ def main(argv=None) -> Dict[str, float]:
         model.bert.use_fused = False          # fp32 requested: plain PyTorch path
     model.bert.unpad = bool(args.unpad)
     arena = ParamArena(model, device=dev)
+    args.fused = fused_program(model, args)
     optimizer = Adam(model.parameters(), lr=args.lr, bias_correction=False)
     arena.bind_optimizer(optimizer)
     scheduler = torch.optim.lr_scheduler.LambdaLR(optimizer, lambda e: 1.0 / (1.0 + 0.05 * e))

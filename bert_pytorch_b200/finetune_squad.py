@@ -7,8 +7,11 @@ Flags, outputs and metrics follow the reference's run_squad.py (:732-857, :1115-
 ``inference_sequences_per_second``, ``exact_match``, ``F1``; the feature cache pickle is named
 ``<train>_<bert_model>_<max_seq>_<stride>_<max_query>``.
 
-Execution differs (H100-first): the encoder runs through the fused sm_90a engine behind an autograd
-bridge; ``--fp16``/``--amp`` select 16-bit compute (bf16 by default on CUDA -- no loss scaling needed;
+Execution differs (H100-first): with bf16 compute (``--bf16``, or ``--fp16``/``--amp`` without ``--loss_scale``) on
+one GPU, every training step and prediction batch runs as the fused sm_90a program of ``BertForQuestionAnswering``
+(``train_step`` / ``predict``: encoder, span head and loss in our kernels, replayed as one CUDA graph; a short last
+batch is filled with inert rows); otherwise the encoder runs through the fused engine behind an autograd bridge.
+``--fp16``/``--amp`` select 16-bit compute (bf16 by default on CUDA -- no loss scaling needed;
 ``--loss_scale`` is honoured for fp16) with the fused multi-tensor Adam kernel (apex FusedAdam contract,
 ``bias_correction=False``) on the flat arena and device-side gradient clipping (no ``.item()`` per
 micro-step, SURVEY O7); without them the fp32 ``BertAdam`` path of the reference is kept.  Data
@@ -119,6 +122,32 @@ def _features_to_tensors(features: List[SQ.InputFeatures], training: bool):
     return TensorDataset(ids, mask, seg, torch.arange(ids.size(0), dtype=torch.long))
 
 
+def fill_batch(batch, batch_size: int, S: int):
+    """A short batch (the loader's host tensors: ids, mask, segments, then the start and end positions of a training
+    batch) filled up to ``batch_size`` rows with inert ones, so that one batch shape (one CUDA graph) serves the whole
+    epoch: one unmasked [PAD] token (id 0, segment 0) and positions S -- the ignored index after the clamp (-1 would
+    clamp to the valid target 0).  Prediction discards the filled rows."""
+    n = batch[0].size(0)
+    k = batch_size - n
+    if k <= 0:
+        return batch
+    ids, mask, seg = batch[:3]
+
+    def pad(t, fill):
+        return torch.cat([t, torch.full((k,) + tuple(t.shape[1:]), fill, dtype=t.dtype)])
+    mask_fill = torch.zeros((k,) + tuple(mask.shape[1:]), dtype=mask.dtype)
+    mask_fill[:, 0] = 1
+    return (pad(ids, 0), torch.cat([mask, mask_fill]), pad(seg, 0), *(pad(t, S) for t in batch[3:]))
+
+
+def fused_program(model, S: int, device, compute_dtype) -> bool:
+    """Whether training and prediction run through the model's fused sm_90a program: bf16 compute on a GPU, and an
+    encoder and sequence length the engine serves."""
+    if compute_dtype != torch.bfloat16 or device.type != "cuda":
+        return False
+    return model.bert._can_fuse(torch.zeros(1, S, dtype=torch.long, device=device))
+
+
 def squad_loss(start_logits, end_logits, start_positions, end_positions):
     """Mean of the start and end cross-entropies; positions outside the window are clamped to an ignored
     index (run_squad.py:1085-1092)."""
@@ -219,6 +248,9 @@ def main(argv=None) -> dict:
         model.bert.use_fused = False
         forward_model = torch.nn.DataParallel(model)
         dll.log(step="PARAMETER", data={"single_process_data_parallel_gpus": torch.cuda.device_count()})
+    # bf16 compute: training steps and prediction batches run as the model's fused program (graph-replayed); the fp16
+    # loss-scaled path, fp32 and the legacy nn.DataParallel mode keep the module path
+    fused = forward_model is ddp and fused_program(model, args.max_seq_length, device, compute_dtype)
 
     optimizer = scheduler = scaler = None
     if args.do_train:
@@ -277,15 +309,21 @@ def main(argv=None) -> dict:
                 if args.max_steps > 0 and global_step >= args.max_steps:      # Q22 fixed
                     done = True
                     break
+                if fused:
+                    batch = fill_batch(batch, args.train_batch_size, args.max_seq_length)
                 ids, mask, seg, sp, ep = (t.to(device, non_blocking=True) for t in batch)
-                with torch.autocast(device_type=device.type, dtype=compute_dtype,
-                                    enabled=compute_dtype != torch.float32):
-                    start_logits, end_logits = forward_model(ids, seg, mask)
-                    loss = squad_loss(start_logits, end_logits, sp, ep)
+                if fused:
+                    loss = model.train_step(ids, seg, mask, sp, ep, grad_scale=1.0 / acc)
+                else:
+                    with torch.autocast(device_type=device.type, dtype=compute_dtype,
+                                        enabled=compute_dtype != torch.float32):
+                        start_logits, end_logits = forward_model(ids, seg, mask)
+                        loss = squad_loss(start_logits, end_logits, sp, ep)
                 if acc > 1:
                     loss = loss / acc
                 boundary = (step + 1) % acc == 0
-                (scaler.scale(loss) if scaler is not None else loss).backward()
+                if not fused:
+                    (scaler.scale(loss) if scaler is not None else loss).backward()
                 if boundary:
                     ddp.sync_gradients()
                     if scaler is not None:
@@ -332,9 +370,15 @@ def main(argv=None) -> dict:
         t0 = time.time()
         with torch.no_grad():
             for ids, mask, seg, idx in loader:
-                with torch.autocast(device_type=device.type, dtype=compute_dtype, enabled=compute_dtype != torch.float32):
-                    s, e = model(ids.to(device), seg.to(device), mask.to(device))
-                s, e = s.float().cpu().tolist(), e.float().cpu().tolist()     # one D2H per batch, not per example
+                if fused:
+                    ids, mask, seg = fill_batch((ids, mask, seg), args.predict_batch_size, args.max_seq_length)
+                    s, e = model.predict(ids.to(device), seg.to(device), mask.to(device), tokens=int(mask.sum()))
+                else:
+                    with torch.autocast(device_type=device.type, dtype=compute_dtype,
+                                        enabled=compute_dtype != torch.float32):
+                        s, e = model(ids.to(device), seg.to(device), mask.to(device))
+                n = idx.numel()
+                s, e = s[:n].float().cpu().tolist(), e[:n].float().cpu().tolist()   # one D2H per batch, not per example
                 for j, i in enumerate(idx.tolist()):
                     results.append(SQ.RawResult(eval_features[i].unique_id, s[j], e[j]))
         time_to_infer = time.time() - t0

@@ -57,6 +57,9 @@ _EMB_LAYER = 1023
 # dropout on the pooled row of the sequence classifier (FusedClassifier): site 4 of the embedding's layer slot.  No
 # encoder layer uses site 4 and the embedding uses site 0, so the stream collides with none of theirs at any depth.
 SITE_CLS = 4
+# dropout on the sequence output under the per-token heads (FusedTokenClassifier): site 5 of the same slot, used by no
+# encoder layer, the embedding or the sequence classifier
+SITE_TOKEN = 5
 
 
 def _stream(layer: int, site: int) -> int:
@@ -64,6 +67,7 @@ def _stream(layer: int, site: int) -> int:
 
 
 CLS_STREAM = _stream(_EMB_LAYER, SITE_CLS)
+TOKEN_STREAM = _stream(_EMB_LAYER, SITE_TOKEN)
 
 
 def _as_tuple(x):
@@ -1105,3 +1109,134 @@ class FusedClassifier(_GraphedProgram):
         seq, _, pk, _ = self._encode(input_ids, segment_ids, input_mask, bucket, train=False)
         _, pooled = self._pooled(seq, self._cls_rows(pk, B, S, seq.device))
         return K.cls_logits(pooled, self.arena.shadow("classifier.weight"), self.model.classifier.bias)
+
+
+class _TokenHeadProgram(_GraphedProgram):
+    """What the per-token head programs share: the head's bf16 weight, fp32 bias and gradient slots, its evaluation
+    program (the forward without dropout, ending in fp32 logits [B, S, N] -- ``bias`` at the masked positions of an
+    unpadded batch), and ``predict`` under graph keys of kind ``eval_kind``."""
+
+    eval_kind = ""
+
+    def __init__(self, model, head: torch.nn.Linear, head_name: str):
+        super().__init__(model)
+        if head.out_features > K.TOKEN_HEAD_MAX_N:
+            raise ValueError(f"{type(self).__name__}: {head.out_features} outputs; the per-token head kernels serve "
+                             f"at most {K.TOKEN_HEAD_MAX_N}")
+        self.head, self.head_name = head, head_name
+
+    def _w(self) -> torch.Tensor:
+        return self.arena.shadow(self.head_name + ".weight")
+
+    @torch.no_grad()
+    def _predict(self, input_ids, segment_ids, input_mask, tokens: Optional[int] = None) -> torch.Tensor:
+        bucket = self._bucket(input_mask, tokens, kfac=False)
+        args = (input_ids, segment_ids, input_mask)
+        run = lambda *a: self._eval_program(*a, bucket=bucket)                                 # noqa: E731
+
+        def go():
+            if not self._eval_graphs_ok():
+                return run(*args)
+            key = self._graph_key(self.eval_kind, args, bucket, False)
+            return self._graphed(key, args, run, train=False, what="evaluation").clone()
+        return self._keeping_fp8_table(go)
+
+    @torch.no_grad()
+    def _eval_program(self, input_ids, segment_ids, input_mask, bucket=None) -> torch.Tensor:
+        B, S = input_ids.shape
+        seq, _, pk, _ = self._encode(input_ids, segment_ids, input_mask, bucket, train=False)
+        logits = K.token_logits(seq, self._w(), self.head.bias, row_map=pk.row_map if pk is not None else None,
+                                mask=input_mask)
+        return logits.view(B, S, -1)
+
+
+class FusedQuestionAnswering(_TokenHeadProgram):
+    """SQuAD fine-tuning and prediction of ``BertForQuestionAnswering`` as one kernel program each.
+
+    Training (``train_step``): encoder forward -> ``token_logits`` (N = 2, no dropout, as in the reference) ->
+    ``span_ce_`` (start / end cross-entropy in place) -> ``token_head_bwd`` -> encoder backward.  Training always runs
+    padded, whatever ``BertModel.unpad`` says: the span softmax normalises over every position, and the encoder outputs
+    of the padded positions cannot be had without computing them.  Prediction (``predict``) honours ``unpad``.  A row
+    whose start and end positions are S (outside [0, S) after the clamp) is inert: a batch filled up to the static batch
+    size with such rows replays the same graph and its loss is that of the real rows."""
+
+    eval_kind = "qa-eval"
+
+    def __init__(self, model):
+        super().__init__(model, model.qa_outputs, "qa_outputs")
+
+    @torch.no_grad()
+    def train_step(self, input_ids, segment_ids, input_mask, start_positions, end_positions,
+                   grad_scale: float = 1.0) -> torch.Tensor:
+        """Forward, loss and backward of one batch: returns the SQuAD loss (a device scalar) and accumulates the
+        gradients, times ``grad_scale``, in the arena."""
+        run = lambda *a, seed=None: self._program(*a, grad_scale, seed=seed)                  # noqa: E731
+        args = (input_ids, segment_ids, input_mask, start_positions, end_positions)
+        if not self._graph_ok():
+            return run(*args)
+        return self._graphed(self._graph_key("qa", args, None, True), args, run, train=True, grad_scale=grad_scale)
+
+    @torch.no_grad()
+    def _program(self, input_ids, segment_ids, input_mask, start_positions, end_positions, grad_scale: float = 1.0,
+                 seed: Optional[int] = None) -> torch.Tensor:
+        seq, sv, _, _ = self._encode(input_ids, segment_ids, input_mask, None, train=True, seed=seed)
+        logits = K.token_logits(seq, self._w(), self.head.bias)
+        loss = torch.zeros(1, dtype=torch.float32, device=seq.device)
+        K.span_ce_(logits, start_positions, end_positions, grad_scale, loss)            # logits <- dlogits
+        d_seq = K.token_head_bwd(logits, seq, self._w(), self.head.weight.grad, self.head.bias.grad)
+        self.engine.backward(sv, d_seq)
+        return loss.squeeze(0)
+
+    def predict(self, input_ids, segment_ids, input_mask, tokens: Optional[int] = None):
+        """fp32 ``(start, end)`` logits, each [B, S], without dropout; unpadded (``BertModel.unpad``, the batch packed
+        into the token bucket of ``tokens``) they are exactly ``bias`` at the masked positions.  Leaves the training
+        state as it was."""
+        out = self._predict(input_ids, segment_ids, input_mask, tokens).permute(2, 0, 1).contiguous()
+        return out[0], out[1]
+
+
+class FusedTokenClassifier(_TokenHeadProgram):
+    """NER fine-tuning and prediction of ``BertForTokenClassification`` as one kernel program each.
+
+    Training (``train_step``): [device packing] -> encoder forward -> ``token_logits`` with dropout
+    ``hidden_dropout_prob`` on the sequence output (stream :data:`TOKEN_STREAM`, the encoder's seed: a replayed graph
+    draws new masks) -> ``token_ce_`` (the masked cross-entropy in place, through the packing's ``row_map``) ->
+    ``token_head_bwd`` -> encoder backward.  Prediction (``predict``): fp32 logits [B, S, N].  A position counts iff its
+    ``attention_mask`` is 1 and its label lies in [0, N): rows of label -100 are inert, so a short batch filled up with
+    them replays the same graph and its loss is that of the real rows."""
+
+    eval_kind = "tok-eval"
+
+    def __init__(self, model):
+        super().__init__(model, model.classifier, "classifier")
+
+    @torch.no_grad()
+    def train_step(self, input_ids, segment_ids, input_mask, labels, grad_scale: float = 1.0,
+                   tokens: Optional[int] = None) -> torch.Tensor:
+        """Forward, loss and backward of one batch: returns the mean cross-entropy over the counted positions (a
+        device scalar) and accumulates the gradients, times ``grad_scale``, in the arena.  Unpadded
+        (``BertModel.unpad``) the batch is packed into the token bucket of ``tokens`` (its unmasked token count, a host
+        int; read back from the device when omitted)."""
+        bucket = self._bucket(input_mask, tokens)
+        run = lambda *a, seed=None: self._program(*a, grad_scale, seed=seed, bucket=bucket)   # noqa: E731
+        args = (input_ids, segment_ids, input_mask, labels)
+        if not self._graph_ok():
+            return run(*args)
+        return self._graphed(self._graph_key("tok", args, bucket, True), args, run, train=True, grad_scale=grad_scale)
+
+    @torch.no_grad()
+    def _program(self, input_ids, segment_ids, input_mask, labels, grad_scale: float = 1.0, seed: Optional[int] = None,
+                 bucket=None) -> torch.Tensor:
+        seq, sv, pk, _ = self._encode(input_ids, segment_ids, input_mask, bucket, train=True, seed=seed)
+        logits = K.token_logits(seq, self._w(), self.head.bias, sv.p_hidden, sv.seed, TOKEN_STREAM)
+        loss = torch.zeros(1, dtype=torch.float32, device=seq.device)
+        K.token_ce_(logits, labels, grad_scale, loss, mask=input_mask, row_map=pk.row_map if pk is not None else None)
+        d_seq = K.token_head_bwd(logits, seq, self._w(), self.head.weight.grad, self.head.bias.grad, sv.p_hidden,
+                                 sv.seed, TOKEN_STREAM)
+        self.engine.backward(sv, d_seq)
+        return loss.squeeze(0)
+
+    def predict(self, input_ids, segment_ids, input_mask, tokens: Optional[int] = None) -> torch.Tensor:
+        """fp32 logits [B, S, N] without dropout (``bias`` at the masked positions when unpadded).  Leaves the training
+        state as it was."""
+        return self._predict(input_ids, segment_ids, input_mask, tokens)

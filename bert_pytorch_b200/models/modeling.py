@@ -779,6 +779,7 @@ class BertForTokenClassification(BertPreTrainedModel):
         self.bert = BertModel(config)
         self.dropout = nn.Dropout(config.hidden_dropout_prob)
         self.classifier = nn.Linear(config.hidden_size, num_labels)
+        self._token_program = None
         self.apply(self.init_bert_weights)
 
     def forward(self, input_ids, token_type_ids=None, attention_mask=None, labels=None):
@@ -794,12 +795,53 @@ class BertForTokenClassification(BertPreTrainedModel):
             return F.cross_entropy(flat_logits, flat_labels)
         return logits
 
+    def token_engine(self):
+        """The fused sm_90a training / prediction program of this model (:class:`~.fused.FusedTokenClassifier`), or
+        ``None`` where it cannot run: more labels than the per-token head kernels serve (64)."""
+        from ..ops.api import TOKEN_HEAD_MAX_N
+        if self.num_labels > TOKEN_HEAD_MAX_N:
+            return None
+        if self._token_program is None:
+            from .fused import FusedTokenClassifier
+            self._token_program = FusedTokenClassifier(self)
+        return self._token_program
+
+    def _fused(self, input_ids):
+        return self.token_engine() if self.bert._can_fuse(input_ids) else None
+
+    def train_step(self, input_ids, token_type_ids, attention_mask, labels, grad_scale: float = 1.0,
+                   tokens: Optional[int] = None) -> torch.Tensor:
+        """Forward, loss and backward of one batch: returns the mean cross-entropy over the positions whose
+        ``attention_mask`` is 1 and whose label lies in [0, num_labels) (every other label, -100 or -1, is ignored; 0
+        when nothing counts) and accumulates the gradients (times ``grad_scale``) into ``.grad``.  Through the fused
+        program (:meth:`~.fused.FusedTokenClassifier.train_step`) where it runs, else the plain PyTorch forward and
+        backward (autocast is the caller's).  ``tokens``: the unmasked token count (a host int) for the unpadded
+        program's bucket."""
+        eng = self._fused(input_ids)
+        if eng is not None:
+            return eng.train_step(input_ids, token_type_ids, attention_mask, labels, grad_scale, tokens=tokens)
+        logits = self(input_ids.long(), None if token_type_ids is None else token_type_ids.long(), attention_mask.long())
+        loss = token_loss(logits, labels, attention_mask)
+        (loss * grad_scale).backward()
+        return loss.detach()
+
+    @torch.no_grad()
+    def predict(self, input_ids, token_type_ids, attention_mask, tokens: Optional[int] = None) -> torch.Tensor:
+        """fp32 logits [B, S, num_labels] without dropout.  Through the fused program
+        (:meth:`~.fused.FusedTokenClassifier.predict`) where it runs, else the plain PyTorch forward in eval mode
+        (autocast is the caller's); ``self.training`` is left as it was."""
+        eng = self._fused(input_ids)
+        if eng is not None:
+            return eng.predict(input_ids, token_type_ids, attention_mask, tokens=tokens)
+        return _eval_forward(self, input_ids, token_type_ids, attention_mask).float()
+
 
 class BertForQuestionAnswering(BertPreTrainedModel):
     def __init__(self, config: BertConfig):
         super().__init__(config)
         self.bert = BertModel(config)
         self.qa_outputs = nn.Linear(config.hidden_size, 2)
+        self._qa_program = None
         self.apply(self.init_bert_weights)
 
     def forward(self, input_ids, token_type_ids=None, attention_mask=None):
@@ -808,6 +850,77 @@ class BertForQuestionAnswering(BertPreTrainedModel):
         logits = _head(self.qa_outputs, seq)                        # K28: own small-N GEMM on an H100
         start, end = logits.split(1, dim=-1)
         return start.squeeze(-1), end.squeeze(-1)
+
+    def qa_engine(self):
+        """The fused sm_90a training / prediction program of this model (:class:`~.fused.FusedQuestionAnswering`)."""
+        if self._qa_program is None:
+            from .fused import FusedQuestionAnswering
+            self._qa_program = FusedQuestionAnswering(self)
+        return self._qa_program
+
+    def _fused(self, input_ids):
+        return self.qa_engine() if self.bert._can_fuse(input_ids) else None
+
+    def train_step(self, input_ids, token_type_ids, attention_mask, start_positions, end_positions,
+                   grad_scale: float = 1.0) -> torch.Tensor:
+        """Forward, loss and backward of one batch: returns the SQuAD loss (:func:`span_loss`) and accumulates the
+        gradients (times ``grad_scale``) into ``.grad``.  Through the fused program
+        (:meth:`~.fused.FusedQuestionAnswering.train_step`, always padded) where it runs, else the plain PyTorch
+        forward and backward (autocast is the caller's)."""
+        eng = self._fused(input_ids)
+        if eng is not None:
+            return eng.train_step(input_ids, token_type_ids, attention_mask, start_positions, end_positions, grad_scale)
+        start, end = self(input_ids.long(), None if token_type_ids is None else token_type_ids.long(),
+                          attention_mask.long())
+        loss = span_loss(start, end, start_positions, end_positions)
+        (loss * grad_scale).backward()
+        return loss.detach()
+
+    @torch.no_grad()
+    def predict(self, input_ids, token_type_ids, attention_mask, tokens: Optional[int] = None):
+        """fp32 ``(start, end)`` logits, each [B, S], without dropout.  Through the fused program
+        (:meth:`~.fused.FusedQuestionAnswering.predict`) where it runs, else the plain PyTorch forward in eval mode
+        (autocast is the caller's); ``self.training`` is left as it was."""
+        eng = self._fused(input_ids)
+        if eng is not None:
+            return eng.predict(input_ids, token_type_ids, attention_mask, tokens=tokens)
+        start, end = _eval_forward(self, input_ids, token_type_ids, attention_mask)
+        return start.float(), end.float()
+
+
+def _eval_forward(model, input_ids, token_type_ids, attention_mask):
+    """``model``'s forward in eval mode (no dropout), ``model.training`` restored afterwards."""
+    was = model.training
+    model.eval()
+    try:
+        return model(input_ids.long(), None if token_type_ids is None else token_type_ids.long(), attention_mask.long())
+    finally:
+        model.train(was)
+
+
+def span_loss(start_logits, end_logits, start_positions, end_positions):
+    """The SQuAD loss (run_squad.py:1085-1092): positions are clamped to [0, S] and S is ignored; the mean start and
+    the mean end cross-entropy, each over its own non-ignored sequences, averaged.  A column with no such sequence
+    contributes 0 (and a zero gradient) instead of NaN."""
+    S = start_logits.size(1)
+    total = 0.0
+    for logits, pos in ((start_logits, start_positions), (end_logits, end_positions)):
+        y = pos.long().to(logits.device).clamp(0, S)
+        n = (y != S).sum().clamp(min=1)
+        total = total + F.cross_entropy(logits.float(), y, ignore_index=S, reduction="sum") / n
+    return total / 2
+
+
+def token_loss(logits, labels, attention_mask):
+    """The NER loss: the mean cross-entropy over the positions whose ``attention_mask`` is 1 and whose label lies in
+    [0, num_labels) (src/modeling.py:1259-1268 masks by attention_mask; -100 and -1 are ignored); 0 with a zero
+    gradient when no position counts."""
+    N = logits.size(-1)
+    flat = logits.reshape(-1, N).float()
+    y = labels.reshape(-1).long().to(flat.device)
+    keep = (attention_mask.reshape(-1).to(flat.device) == 1) & (y >= 0) & (y < N)
+    y = torch.where(keep, y, torch.full_like(y, -100))
+    return F.cross_entropy(flat, y, ignore_index=-100, reduction="sum") / keep.sum().clamp(min=1)
 
 
 class BertPretrainingCriterion(nn.Module):

@@ -415,6 +415,74 @@ def cls_logits(pooled: torch.Tensor, w: torch.Tensor, bias: torch.Tensor) -> tor
     return out
 
 
+TOKEN_HEAD_MAX_N = 64   # the widest per-token head the token_* kernels serve (QA: 2, NER: len(labels) + 1)
+
+
+def _i32(t: torch.Tensor) -> torch.Tensor:
+    return t.reshape(-1).to(torch.int32).contiguous()
+
+
+def token_logits(seq: torch.Tensor, w: torch.Tensor, bias: torch.Tensor, p_drop: float = 0.0, seed: int = 0,
+                 stream: int = 0, row_map: Optional[torch.Tensor] = None,
+                 mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Per-token head forward: fp32 logits [M, N] = dropout(``seq``) @ ``w``^T + ``bias`` for the bf16 [M, H] sequence
+    output (H % 8 == 0) and a bf16 [N, H] weight, 1 <= N <= 64.  Dropout ``p_drop`` draws Philox ``(seed, stream)`` at
+    element ``row * H + i`` (:func:`bert_pytorch_b200.utils.philox.keep_bits`).  With ``row_map`` (int32 [B * S] from
+    :func:`pack_tokens`, ``seq`` the packed rows) and the batch's attention ``mask`` the result is unpacked to
+    [B * S, N], ``bias`` at the masked positions."""
+    out = torch.empty(seq.size(0) if seq.dim() == 2 else 0, w.size(0) if w.dim() == 2 else 0, dtype=torch.float32,
+                      device=seq.device)
+    extension().token_logits(seq, w, bias, p_drop, seed, stream, out)
+    _count()
+    if row_map is None:
+        return out
+    full = torch.empty(row_map.numel(), out.size(1), dtype=torch.float32, device=seq.device)
+    extension().token_unpack(out, row_map, _i32(mask), bias, full)
+    _count()
+    return full
+
+
+def token_ce_(logits: torch.Tensor, labels: torch.Tensor, grad_scale: float, loss_out: torch.Tensor,
+              mask: Optional[torch.Tensor] = None, row_map: Optional[torch.Tensor] = None) -> None:
+    """NER loss, in place: ``logits`` (fp32 [R, N]) <- d loss / d logits times ``grad_scale``, ``loss_out`` += the mean
+    cross-entropy over the counted positions: ``mask == 1`` (every position without a mask) and ``0 <= label < N``
+    (-100, -1 and labels >= N are ignored).  With ``row_map`` (from :func:`pack_tokens`) position p reads packed row
+    ``row_map[p]``; rows that no counted position maps to get a zero gradient.  The count stays on the device; with no
+    counted position the loss and every gradient are 0.  Deterministic mode: per-CTA loss sums added by ordered_sum."""
+    det = deterministic()
+    extension().token_ce(logits, _i32(labels), None if mask is None else _i32(mask),
+                         None if row_map is None else _i32(row_map), grad_scale, loss_out, det)
+    _count(3 if det else 2)
+
+
+def span_ce_(logits: torch.Tensor, start_positions: torch.Tensor, end_positions: torch.Tensor, grad_scale: float,
+             loss_out: torch.Tensor) -> None:
+    """SQuAD loss, in place on the padded fp32 logits [B * S, 2] (start, end): per sequence a softmax over its S
+    positions for each column; positions are clamped to [0, S] and S is ignored.  ``loss_out`` += (mean start CE + mean
+    end CE) / 2, each mean over its own non-ignored sequences (0 without any); ``logits`` <- d loss / d logits times
+    ``grad_scale``."""
+    B = start_positions.numel()
+    if B == 0 or logits.dim() != 2 or logits.size(0) % B != 0:
+        raise ValueError(f"span_ce_: logits {tuple(logits.shape)} is not [B * S, 2] for B = {B}")
+    det = deterministic()
+    extension().span_ce(logits, _i32(start_positions), _i32(end_positions), logits.size(0) // B, grad_scale, loss_out,
+                        det)
+    _count(2 if det else 1)
+
+
+def token_head_bwd(dlogits: torch.Tensor, seq: torch.Tensor, w: torch.Tensor, dw: torch.Tensor, db: torch.Tensor,
+                   p_drop: float = 0.0, seed: int = 0, stream: int = 0) -> torch.Tensor:
+    """Per-token head backward: returns d_seq bf16 [M, H] = (``dlogits`` @ ``w``) * keep / (1 - p), and accumulates
+    ``dw`` (fp32 [N, H]) += dlogits^T @ dropout(seq) and ``db`` (fp32 [N]) += the column sums of dlogits -- per CTA over
+    fixed 512-row partitions, then one atomic per CTA and element, or (deterministic mode) the partitions' partials
+    added in order by ordered_sum.  The keep bits are :func:`token_logits`' for the same ``(seed, stream)``."""
+    dseq = torch.empty_like(seq)
+    det = deterministic()
+    extension().token_head_bwd(dlogits, seq, w, dw, db, p_drop, seed, stream, dseq, det)
+    _count(3 if det else 1)
+    return dseq
+
+
 def softmax_ce_(logits: torch.Tensor, targets: torch.Tensor, count: torch.Tensor, grad_scale: float,
                 loss_out: torch.Tensor) -> None:
     """In place: logits <- d loss / d logits (scaled); loss_out += mean CE over valid targets."""

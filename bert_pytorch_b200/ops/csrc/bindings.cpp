@@ -720,6 +720,120 @@ void cls_logits(Tensor pooled, Tensor w, Tensor bias, Tensor logits) {
                    logits.data_ptr<float>(), cur_stream());
 }
 
+// per-token heads: seq bf16 [M, H] (H % 8 == 0), w bf16 [N, H] with 1 <= N <= 64, fp32 bias [N], all on one device
+inline void check_token_head(const Tensor& seq, const Tensor& w, const Tensor& bias, double p_drop, const char* name) {
+  check_bf16(seq, "seq"); check_bf16(w, "w");
+  TORCH_CHECK(seq.dim() == 2 && seq.is_contiguous() && seq.size(1) % 8 == 0, name,
+              ": seq must be a contiguous [M, H] with H % 8 == 0");
+  TORCH_CHECK(w.dim() == 2 && w.is_contiguous() && w.size(0) >= 1 && w.size(0) <= 64 && w.size(1) == seq.size(1), name,
+              ": w must be a contiguous [N, H] with 1 <= N <= 64");
+  TORCH_CHECK(w.device() == seq.device(), name, ": w must be on seq's device");
+  TORCH_CHECK(bias.is_cuda() && bias.device() == seq.device() && bias.scalar_type() == at::kFloat && bias.is_contiguous() &&
+              bias.numel() == w.size(0), name, ": bias must be a contiguous fp32 CUDA tensor [N] on seq's device");
+  TORCH_CHECK(p_drop >= 0.0 && p_drop < 1.0, name, ": p_drop must lie in [0, 1)");
+}
+
+inline void check_f32_on(const Tensor& t, const Tensor& like, int64_t numel, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.device() == like.device() && t.scalar_type() == at::kFloat && t.is_contiguous() &&
+              t.numel() == numel, name, " must be a contiguous fp32 CUDA tensor of ", numel, " elements on the batch's device");
+}
+
+void token_logits(Tensor seq, Tensor w, Tensor bias, double p_drop, int64_t seed, int64_t stream_id, Tensor out) {
+  check_token_head(seq, w, bias, p_drop, "token_logits");
+  const int64_t M = seq.size(0), H = seq.size(1), N = w.size(0);
+  check_f32_on(out, seq, M * N, "token_logits: out");
+  c10::cuda::CUDAGuard guard(seq.device());
+  b200::token_logits(seq.data_ptr(), w.data_ptr(), bias.data_ptr<float>(), (int)M, (int)H, (int)N, mk_seed(seed),
+                     (unsigned)stream_id, (float)p_drop, out.data_ptr<float>(), cur_stream());
+}
+
+void token_unpack(Tensor logits, Tensor row_map, Tensor mask, Tensor bias, Tensor out) {
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.is_contiguous() && logits.dim() == 2,
+              "token_unpack: logits must be a contiguous fp32 CUDA tensor [T, N]");
+  const int64_t N = logits.size(1), P = row_map.numel();
+  check_i32(row_map, logits, P, "token_unpack: row_map");
+  check_i32(mask, logits, P, "token_unpack: mask");
+  check_f32_on(bias, logits, N, "token_unpack: bias");
+  check_f32_on(out, logits, P * N, "token_unpack: out");
+  c10::cuda::CUDAGuard guard(logits.device());
+  b200::token_unpack(logits.data_ptr<float>(), row_map.data_ptr<int>(), mask.data_ptr<int>(), bias.data_ptr<float>(),
+                     (int)P, (int)N, out.data_ptr<float>(), cur_stream());
+}
+
+// logits fp32 [R, N] (in place), labels int32 [P], mask int32 [P] (optional), row_map int32 [P] (optional; without it
+// P == R), loss fp32
+void token_ce(Tensor logits, Tensor labels, c10::optional<Tensor> mask, c10::optional<Tensor> row_map, double grad_scale,
+              Tensor loss_out, bool deterministic) {
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.is_contiguous() && logits.dim() == 2 &&
+              logits.size(1) >= 1 && logits.size(1) <= 64, "token_ce: logits must be a contiguous fp32 CUDA tensor [R, N], "
+              "1 <= N <= 64");
+  const int64_t R = logits.size(0), N = logits.size(1), P = labels.numel();
+  check_i32(labels, logits, P, "token_ce: labels");
+  const int* mask_p = nullptr;
+  const int* rm_p = nullptr;
+  if (mask.has_value() && mask->defined()) {
+    check_i32(*mask, logits, P, "token_ce: mask");
+    mask_p = mask->data_ptr<int>();
+  }
+  if (row_map.has_value() && row_map->defined()) {
+    check_i32(*row_map, logits, P, "token_ce: row_map");
+    rm_p = row_map->data_ptr<int>();
+  } else {
+    TORCH_CHECK(P == R, "token_ce: without a row_map there must be one label per logits row");
+  }
+  TORCH_CHECK(loss_out.is_cuda() && loss_out.device() == logits.device() && loss_out.scalar_type() == at::kFloat &&
+              loss_out.numel() >= 1, "token_ce: loss_out must be an fp32 CUDA tensor");
+  TORCH_CHECK(R < (int64_t(1) << 31) && P < (int64_t(1) << 31), "token_ce: too many rows");
+  c10::cuda::CUDAGuard guard(logits.device());
+  Tensor idx = at::empty({R + 1}, labels.options());
+  Tensor part;
+  if (deterministic) part = f32_workspace(logits, b200::token_ce_parts((int)R));
+  b200::token_ce(logits.data_ptr<float>(), labels.data_ptr<int>(), mask_p, rm_p, (int)P, (int)R, (int)N, (float)grad_scale,
+                 loss_out.data_ptr<float>(), idx.data_ptr<int>(), deterministic ? part.data_ptr<float>() : nullptr,
+                 cur_stream());
+}
+
+// logits fp32 [B * S, 2] (in place), start / end int32 [B]
+void span_ce(Tensor logits, Tensor start, Tensor end, int64_t S, double grad_scale, Tensor loss_out, bool deterministic) {
+  TORCH_CHECK(S >= 1, "span_ce: S must be positive");
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.is_contiguous() && logits.dim() == 2 &&
+              logits.size(1) == 2 && logits.size(0) % S == 0, "span_ce: logits must be a contiguous fp32 CUDA tensor "
+              "[B * S, 2]");
+  const int64_t B = logits.size(0) / S;
+  check_i32(start, logits, B, "span_ce: start_positions");
+  check_i32(end, logits, B, "span_ce: end_positions");
+  TORCH_CHECK(loss_out.is_cuda() && loss_out.device() == logits.device() && loss_out.scalar_type() == at::kFloat &&
+              loss_out.numel() >= 1, "span_ce: loss_out must be an fp32 CUDA tensor");
+  c10::cuda::CUDAGuard guard(logits.device());
+  Tensor part;
+  if (deterministic) part = f32_workspace(logits, B);
+  b200::span_ce(logits.data_ptr<float>(), start.data_ptr<int>(), end.data_ptr<int>(), (int)B, (int)S, (float)grad_scale,
+                loss_out.data_ptr<float>(), deterministic ? part.data_ptr<float>() : nullptr, cur_stream());
+}
+
+void token_head_bwd(Tensor dlogits, Tensor seq, Tensor w, Tensor dw, Tensor db, double p_drop, int64_t seed,
+                    int64_t stream_id, Tensor dseq, bool deterministic) {
+  TORCH_CHECK(p_drop >= 0.0 && p_drop < 1.0, "token_head_bwd: p_drop must lie in [0, 1)");
+  check_bf16(seq, "seq"); check_bf16(w, "w"); check_bf16(dseq, "dseq");
+  TORCH_CHECK(seq.dim() == 2 && seq.is_contiguous() && seq.size(1) % 8 == 0,
+              "token_head_bwd: seq must be a contiguous [M, H] with H % 8 == 0");
+  const int64_t M = seq.size(0), H = seq.size(1);
+  TORCH_CHECK(w.dim() == 2 && w.is_contiguous() && w.size(0) >= 1 && w.size(0) <= 64 && w.size(1) == H &&
+              w.device() == seq.device(), "token_head_bwd: w must be a contiguous [N, H] with 1 <= N <= 64 on seq's device");
+  const int64_t N = w.size(0);
+  check_f32_on(dlogits, seq, M * N, "token_head_bwd: dlogits");
+  check_f32_on(dw, seq, N * H, "token_head_bwd: dw");
+  check_f32_on(db, seq, N, "token_head_bwd: db");
+  TORCH_CHECK(dseq.device() == seq.device() && dseq.is_contiguous() && dseq.sizes() == seq.sizes(),
+              "token_head_bwd: dseq must be a contiguous tensor of seq's shape");
+  c10::cuda::CUDAGuard guard(seq.device());
+  Tensor ws;
+  if (deterministic) ws = f32_workspace(dw, (int64_t)b200::token_head_bwd_parts((int)M) * (N * H + N));
+  b200::token_head_bwd(dlogits.data_ptr<float>(), seq.data_ptr(), w.data_ptr(), (int)M, (int)H, (int)N, mk_seed(seed),
+                       (unsigned)stream_id, (float)p_drop, dseq.data_ptr(), dw.data_ptr<float>(), db.data_ptr<float>(),
+                       deterministic ? ws.data_ptr<float>() : nullptr, cur_stream());
+}
+
 // evaluation metrics: rows fp32 [R, 3] ({loss, correct, valid} per row), sums fp32 [3] += their column sums (in order)
 inline void check_eval_out(const Tensor& rows, const Tensor& sums, int64_t R, const Tensor& like, const char* name) {
   TORCH_CHECK(rows.is_cuda() && rows.device() == like.device() && rows.scalar_type() == at::kFloat && rows.is_contiguous() &&
@@ -842,6 +956,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("nsp_head", &nsp_head);
   m.def("cls_head", &cls_head);
   m.def("cls_logits", &cls_logits);
+  m.def("token_logits", &token_logits);
+  m.def("token_unpack", &token_unpack);
+  m.def("token_ce", &token_ce);
+  m.def("span_ce", &span_ce);
+  m.def("token_head_bwd", &token_head_bwd);
   m.def("mlm_eval", &mlm_eval);
   m.def("nsp_eval", &nsp_eval);
   m.def("mt_l2norm", &mt_l2norm);

@@ -146,6 +146,28 @@ void cls_head(const void* pooled_bf16, const void* w_bf16, const float* bias, co
 void cls_logits(const void* pooled_bf16, const void* w_bf16, const float* bias, int B, int H, int C, float* logits,
                 cudaStream_t st);
 
+// loss.cu: per-token heads (SQuAD, NER).  seq / w bf16 [M, H] / [N, H], H % 8 == 0, 1 <= N <= 64; fp32 logits [M, N].
+// Dropout p_drop on the seq elements (Philox stream `stream`, element row * H + i).
+void token_logits(const void* seq_bf16, const void* w_bf16, const float* bias, int M, int H, int N, Seed seed,
+                  unsigned int stream, float p_drop, float* logits, cudaStream_t st);
+// out [P, N] = logits[row_map[p]], or bias where mask[p] == 0
+void token_unpack(const float* logits, const int* row_map, const int* mask, const float* bias, int P, int N, float* out,
+                  cudaStream_t st);
+// in place: logits [R, N] <- d loss / d logits; loss_out += the mean CE over the counted positions p < P (mask[p] == 1
+// or no mask, 0 <= labels[p] < N; row row_map[p] or p).  idx_ws int32 [R + 1]; part [token_ce_parts(R)]: deterministic.
+int token_ce_parts(int R);
+void token_ce(float* logits, const int* labels, const int* mask, const int* row_map, int P, int R, int N,
+              float grad_scale, float* loss_out, int* idx_ws, float* part, cudaStream_t st);
+// in place on logits [B * S, 2] (start, end): span cross-entropy with positions clamped to [0, S], S ignored.
+// part [B]: deterministic mode.
+void span_ce(float* logits, const int* start, const int* end, int B, int S, float grad_scale, float* loss_out,
+             float* part, cudaStream_t st);
+// d_seq bf16 [M, H] = (dlogits . W) * keep / (1 - p); dw [N, H] += dlogits^T . dropout(seq); db [N] += column sums.
+// ws [parts * (N H + N)], parts = token_head_bwd_parts(M): deterministic mode (per-partition partials, ordered_sum).
+int token_head_bwd_parts(int M);
+void token_head_bwd(const float* dlogits, const void* seq_bf16, const void* w_bf16, int M, int H, int N, Seed seed,
+                    unsigned int stream, float p_drop, void* dseq_bf16, float* dw, float* db, float* ws, cudaStream_t st);
+
 // loss.cu: evaluation metrics, forward only.  rows [R, 3] receives {loss, correct, valid} of every row ({0, 0, 0} for an
 // ignored one); sums [3] += the column sums of rows, added by ordered_sum (no atomics, the same bits in every mode).
 // mlm_eval: bf16 logits [R, V] (V % 8 == 0, row stride ld), targets int32 (< 0: ignored).  nsp_eval: pooled bf16 [B, H],
